@@ -250,14 +250,15 @@ int launch_read_entries(Table& t, const int* slot, size_t n, float* scal, int* h
 // ---- GPU localizer (kernels_localize.cu): Localizer::Compact + the CSC view from one radix sort ----
 size_t localize_sort_tmp_bytes(size_t nnz);
 // hi32: sort on the upper 32 key bits only (the caller knows the lower 32 are zero: ids < 2^32); verified on the device
-int launch_localize_keys(const uint64_t* ids, size_t nnz, uint64_t max_index, unsigned long long* rkeys,
-                         uint32_t* pos, unsigned long long* or_all, const uint64_t* offset, size_t nrows,
-                         uint32_t* nnz_row, bool hi32, cudaStream_t s);
-int launch_localize_sort(const unsigned long long* rkeys, const uint32_t* pos, size_t nnz, int begin_bit, bool hi32,
-                         unsigned long long* skeys, uint32_t* spos, int* head, int* rank1, void* tmp,
-                         size_t tmp_bytes, const uint32_t* nnz_row, const float* value, uint64_t* keys_out,
-                         int* col_start, int* col_end, uint32_t* lidx_out, void* occ_sorted,
-                         unsigned long long* scal /* {or_all, n_unique} */, DevProgress* prog, cudaStream_t s);
+// pay / spay: 8 bytes per nnz, the sort payload (and on the 64-bit-key path the row of every nnz); see
+// kernels_localize.cu.  offset must describe the nnz ids as CSR: positions no row covers are not localized.
+int launch_localize_keys(const uint64_t* ids, size_t nnz, uint64_t max_index, unsigned long long* rkeys, void* pay,
+                         unsigned long long* or_all, const uint64_t* offset, size_t nrows, bool hi32, cudaStream_t s);
+int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_t nnz, int begin_bit,
+                         bool hi32, unsigned long long* skeys, void* spay, void* tmp, size_t tmp_bytes,
+                         const float* value, uint64_t* keys_out, int* col_start, int* col_end, uint32_t* lidx_out,
+                         void* occ_sorted, unsigned long long* scal /* {or_all, n_unique} */, DevProgress* prog,
+                         cudaStream_t s);
 int launch_cnt_from_cols(const int* col_start, const int* col_end, size_t n, float* cnt, cudaStream_t s);
 
 // ---- sorted (atomic-free, deterministic) gradient reduction ----

@@ -402,11 +402,8 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
   const size_t n1 = nnz ? nnz : 1;
   DFB_TRY(h->ensure(h->l_rkeys, n1 * 8));
   DFB_TRY(h->ensure(h->l_skeys, n1 * 8));
-  DFB_TRY(h->ensure(h->l_pos, n1 * 4));
-  DFB_TRY(h->ensure(h->l_spos, n1 * 4));
-  DFB_TRY(h->ensure(h->l_head, n1 * 4));
-  DFB_TRY(h->ensure(h->l_rank, n1 * 4));
-  DFB_TRY(h->ensure(h->l_nnzrow, n1 * 4));
+  DFB_TRY(h->ensure(h->l_pay, n1 * 8));
+  DFB_TRY(h->ensure(h->l_spay, n1 * 8));
   DFB_TRY(h->ensure(h->l_tmp, localize_sort_tmp_bytes(nnz)));
   DFB_TRY(h->ensure(L.scal, 16));
   DFB_TRY(h->ensure(L.keys, n1 * 8));
@@ -436,7 +433,7 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
   }
   const bool hi32 = begin_bit >= 32;       // only the upper 32 key bits can be set: 32-bit sort keys
   h->launches += launch_localize_keys(d_ids, nnz, max_index, h->l_rkeys.as<unsigned long long>(),
-                                      h->l_pos.as<uint32_t>(), scal, d_off, nrows, h->l_nnzrow.as<uint32_t>(), hi32, s);
+                                      h->l_pay.p, scal, d_off, nrows, hi32, s);
   if (begin_bit < 0) {
     DFB_CUDA(h, cudaMemcpyAsync(h->h_scal, scal, 8, cudaMemcpyDeviceToHost, s));
     DFB_CUDA(h, cudaStreamSynchronize(s));
@@ -451,10 +448,9 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
     }
   }
   {
-    int nl = launch_localize_sort(h->l_rkeys.as<unsigned long long>(), h->l_pos.as<uint32_t>(), nnz, begin_bit, hi32,
-                                  h->l_skeys.as<unsigned long long>(), h->l_spos.as<uint32_t>(),
-                                  h->l_head.as<int>(), h->l_rank.as<int>(), h->l_tmp.p, h->l_tmp.bytes,
-                                  h->l_nnzrow.as<uint32_t>(), d_val, L.keys.as<uint64_t>(),
+    int nl = launch_localize_sort(h->l_rkeys.as<unsigned long long>(), h->l_pay.p, nnz, begin_bit, hi32,
+                                  h->l_skeys.as<unsigned long long>(), h->l_spay.p, h->l_tmp.p, h->l_tmp.bytes, d_val,
+                                  L.keys.as<uint64_t>(),
                                   L.col_start.as<int>(), L.col_end.as<int>(), L.lidx.as<uint32_t>(),
                                   L.occ_sorted.p, scal, h->tab.prog, s);
     if (nl < 0) return h->fail(DFB_ERR_CUDA, "radix sort / scan of the GPU localizer failed (temporary storage)");
@@ -517,6 +513,9 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
 int dfbh::check_csr(dfb_engine* h, size_t nrows, const uint64_t* offset) {
   if (nrows && !offset) return h->fail(DFB_ERR_INVALID, "offset is NULL");
   if (nrows && offset[0] != 0) return h->fail(DFB_ERR_INVALID, "offset[0] must be 0 (fm_loss.h:88 assumes it)");
+  // nnz is offset[nrows]: rows must not run backwards, or the kernels would index outside the nnz arrays
+  for (size_t r = 0; r < nrows; ++r)
+    if (offset[r + 1] < offset[r]) return h->fail(DFB_ERR_INVALID, "offset must be non-decreasing");
   return 0;
 }
 using dfbh::check_csr;
@@ -610,8 +609,11 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
   if ((e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
   if ((e = cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
-  // (default priority: on one GPU a high-priority localizer takes SM slots from the latency-bound lookup / gather
-  // kernels of the current step and costs ~4 %, measured; the sharded store's worker stream does get priority)
+  // Default priority.  On one GPU a high-priority localizer takes SM slots from the latency-bound lookup / gather
+  // kernels of the current step and costs ~4 %, measured.  Holding it back until the update stage starts (HBM-bound,
+  // short-lived CTAs) and then giving it the greatest priority put 91 % of its kernel time under the update, but the
+  // update grew from 3.05 to 3.75 ms: the two share HBM, and the step got 2.3 % slower (H100 SXM, 700 W).  The
+  // sharded store's worker stream does get priority.
   if ((e = cudaStreamCreateWithFlags(&h->loc_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
   for (auto& L : h->loc) {
     if ((e = cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
@@ -671,7 +673,7 @@ int dfb_destroy(dfb_handle h) {
     if (L.consumed) cudaEventDestroy(L.consumed);
   }
   if (h->loc_stream) cudaStreamDestroy(h->loc_stream);
-  DevBuf* bufs[] = {&h->u_wv, &h->l_rkeys, &h->l_skeys, &h->l_pos, &h->l_spos, &h->l_head, &h->l_rank, &h->l_nnzrow,
+  DevBuf* bufs[] = {&h->u_wv, &h->l_rkeys, &h->l_skeys, &h->l_pay, &h->l_spay,
                     &h->hot_map, &h->hot_info, &h->hot_part, &h->hot_ps, &h->hot_cnt, &h->l_tmp, &h->auc_tmp, &h->pxv, &h->p_row, &h->occ, &h->occ_sorted, &h->lidx_sorted, &h->col_start, &h->col_end,
                     &h->keys, &h->cnt, &h->slot, &h->u_w, &h->u_vrow, &h->flags, &h->pos, &h->lens, &h->cub,
                     &h->gw, &h->gxxp, &h->gV, &h->pred, &h->vals, &h->auc_k, &h->auc_v, &h->a_off, &h->a_idx,

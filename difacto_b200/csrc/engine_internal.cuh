@@ -46,7 +46,7 @@ struct dfb_engine {
   DevBuf auc_k, auc_v, auc_tmp;
   DevBuf pxv, p_row, occ, occ_sorted, lidx_sorted, col_start, col_end;
   DevBuf hot_map, hot_info, hot_part, hot_ps, hot_cnt;
-  DevBuf l_rkeys, l_skeys, l_pos, l_spos, l_head, l_rank, l_nnzrow, l_tmp;
+  DevBuf l_rkeys, l_skeys, l_pay, l_spay, l_tmp;
   // outputs of the GPU localizer, double-buffered: the localizer of batch t+1 runs on loc_stream
   // while the step of batch t (which reads set t) runs on the main stream
   struct LocSet {

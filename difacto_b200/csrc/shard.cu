@@ -466,8 +466,8 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   // may be waiting for the very step this rank has not finished enqueuing (ranks that are threads of one process).
   {
     const size_t n1 = max_nnz, B = max_rows;
-    DevBuf* nnz8[] = {&h->l_rkeys, &h->l_skeys, &sh->L.keys, &sh->L.occ_sorted};
-    DevBuf* nnz4[] = {&h->l_pos, &h->l_spos, &h->l_head, &h->l_rank, &h->l_nnzrow, &sh->L.lidx, &sh->L.cnt, &sh->L.col_end};
+    DevBuf* nnz8[] = {&h->l_rkeys, &h->l_skeys, &h->l_pay, &h->l_spay, &sh->L.keys, &sh->L.occ_sorted};
+    DevBuf* nnz4[] = {&sh->L.lidx, &sh->L.cnt, &sh->L.col_end};
     for (auto* b : nnz8) if ((rc = h->ensure(*b, n1 * 8))) return fail(rc);
     for (auto* b : nnz4) if ((rc = h->ensure(*b, n1 * 4))) return fail(rc);
     HotWs hws;
