@@ -36,9 +36,12 @@ struct Params {
 struct DevProgress {
   double loss, penalty, auc;
   unsigned long long nrows, new_keys, new_vrows;
-  int err;        // sticky dfb_status raised by a kernel (capacity, invalid lens ...)
+  int err;        // sticky dfb_status raised by a kernel (capacity, invalid lens ...), or kErrIdRange
   int pad;
 };
+// DevProgress::err of a raw batch the GPU localizer dropped because its ids fall outside the sorted bit range;
+// reported to the caller as DFB_ERR_INVALID with a message that names the range
+constexpr int kErrIdRange = -100;
 
 // device-resident mutable scalars of the table
 struct TableState {
@@ -170,6 +173,10 @@ struct FmBatch {
   // CTA walks one row (0 = one warp per row whatever its length); nnz_hint = the batch's nnz when the host knows it
   unsigned long_nnz;
   size_t nnz_hint;
+  // the device-side key count of a batch the GPU localizer produced (nullptr: none).  0 there (with nnz > 0) means
+  // the localizer dropped the batch: the kernels then return at once, without reading the batch's ranks, and the
+  // forward raises kErrIdRange into prog
+  const unsigned long long* dev_nkeys;
 };
 
 // true when launch_fm would take the 16-byte-lane fast path for this V_dim / view
@@ -240,8 +247,11 @@ int launch_lens_scan(const int* lens, size_t n, int* pos, void* cub_tmp, size_t 
                      cudaStream_t s);
 // Loss::Evaluate / BinClassMetric::AUC on device; results added to prog (or written to out)
 int launch_evaluate(const float* label, const float* pred, size_t n, double* out, cudaStream_t s);
+// dev_nkeys: as FmBatch::dev_nkeys (a dropped batch adds nothing), or nullptr
 int launch_auc(const float* label, const float* pred, size_t n, float* key_tmp2, float* val_tmp2,
-               void* cub_tmp, size_t cub_bytes, double* out_add, cudaStream_t s);
+               void* cub_tmp, size_t cub_bytes, double* out_add, const unsigned long long* dev_nkeys, cudaStream_t s);
+// raises a dfb_status (or kErrIdRange) into prog, in stream order
+int launch_raise_err(DevProgress* prog, int code, cudaStream_t s);
 int launch_restore(Table& t, const uint64_t* keys, size_t n, const float* scal, const int* vrow,
                    unsigned long long n_vrows, unsigned seed, cudaStream_t s);
 int launch_read_entries(Table& t, const int* slot, size_t n, float* scal, int* hasv, float* V,
@@ -257,7 +267,8 @@ int launch_localize_keys(const uint64_t* ids, size_t nnz, uint64_t max_index, un
 int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_t nnz, int begin_bit,
                          bool hi32, unsigned long long* skeys, void* spay, void* tmp, size_t tmp_bytes,
                          const float* value, uint64_t* keys_out, int* col_start, int* col_end, uint32_t* lidx_out,
-                         void* occ_sorted, unsigned long long* scal /* {or_all, n_unique} */, DevProgress* prog,
+                         void* occ_sorted, unsigned long long* scal /* {or_all, n_unique} */,
+                         DevProgress* prog /* nullptr: a dropped batch (n_unique = 0) is the caller's to report */,
                          cudaStream_t s);
 int launch_cnt_from_cols(const int* col_start, const int* col_end, size_t n, float* cnt, cudaStream_t s);
 

@@ -77,6 +77,14 @@ int check_dev_err(dfb_engine* h) {
     case DFB_ERR_INVALID:
       return h->fail(code, "invalid input detected on device (a CHECK of the reference would have failed: "
                            "lens[i] != V_dim+1, gradient for a key without V, or key == UINT64_MAX)");
+    case kErrIdRange: {
+      const std::string range = h->id_bits > 0
+          ? "id_bits = " + std::to_string(h->id_bits) + ": ids below 2^" + std::to_string(4 * ((h->id_bits + 3) / 4))
+          : std::string("id_bits = 0: the range learned from earlier batches, which widens to these ids for later "
+                        "batches");
+      return h->fail(DFB_ERR_INVALID, "a raw batch was dropped, untrained: its ids do not fit in the id range the GPU "
+                                      "localizer sorts (" + range + ")");
+    }
     case DFB_ERR_TIMEOUT:
       return h->fail(code, "a rank of the sharded store did not reach this step within shard_timeout_ms (peer crashed, ran out "
                            "of data without calling the step with nrows = 0, or the ranks' hosts deadlocked)");
@@ -282,6 +290,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   b.pred_in = nullptr; b.pred_io = h->pred.as<float>(); b.pred_acc = 0;
   b.V_dim = h->prm.V_dim; b.train = is_train; b.prog = h->tab.prog;
   b.long_nnz = (unsigned)h->long_row_nnz; b.nnz_hint = nnz;
+  b.dev_nkeys = dU;      // 0 keys for nnz > 0: the localizer dropped the batch; every kernel below then does nothing
   if (sorted) {
     b.emit = 1; b.p_out = h->p_row.as<float>(); b.pxv_out = h->pxv.as<float>();
     b.occ_row = csc_ready ? nullptr : h->occ.as<uint32_t>();
@@ -310,7 +319,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     }
     StageTimer tm(h, 2);
     h->launches += launch_auc(d_lab, h->pred.as<float>(), nrows, h->auc_k.as<float>(),
-                              h->auc_v.as<float>(), h->auc_tmp.p, h->auc_tmp.bytes, &h->tab.prog->auc, as);
+                              h->auc_v.as<float>(), h->auc_tmp.p, h->auc_tmp.bytes, &h->tab.prog->auc, dU, as);
     if (side) {
       DFB_CUDA(h, cudaEventRecord(h->ev_auc_done, as));
       auc_pending = true;
@@ -388,14 +397,15 @@ int lowest_bit(unsigned long long or_all) {
 // Localizer::Compact on the device.  Leaves the unique keys, the remapped CSR index and the CSC view
 // (occ_sorted / col_start / col_end; col_start has U+1 entries) in L.  The radix sort only visits the key
 // bits that are not constant zero; which bits those are is either given (id_bits: ids < 2^id_bits fill the
-// top nibbles of the reversed key), or learned: the first batch is measured with one 8-byte D2H sync, later
-// batches reuse the range (verified on the device; earlier batches' OR masks are read back without waiting
-// and can only widen it); exact_range measures every batch (the synchronous entry points, which wait for
-// the step anyway).  With need_host_U the unique-key count is also synchronised to the host, otherwise it
+// top nibbles of the reversed key, rounded up to whole nibbles), or learned: the first batch is measured with one
+// 8-byte D2H sync, later batches reuse the range (verified on the device; earlier batches' OR masks are read back
+// without waiting and can only widen it); exact_range measures every batch of an engine without id_bits (the
+// synchronous entry points, which wait for the step anyway).  A batch the range does not cover is dropped (see
+// engine_internal.cuh).  With need_host_U the unique-key count is also synchronised to the host, otherwise it
 // stays on the device (L.dU()) and *U_out is the capacity nnz.
 int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                        const float* d_val, uint64_t max_index, dfb_engine::LocSet& L, cudaStream_t s,
-                       bool need_host_U, bool exact_range, size_t* U_out) {
+                       bool need_host_U, bool exact_range, size_t* U_out, DevProgress* drop_prog, bool standalone) {
   *U_out = 0;
   if (nnz > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "batch too large");   // localizer.cc:19-20
   if (max_index == 0) return h->fail(DFB_ERR_INVALID, "max_index must be > 0");
@@ -419,7 +429,8 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
   }
   // ---- the bit range of the sort (known before the keys are produced, unless this batch must be measured) ----
   int begin_bit = -1;
-  const bool restricted = max_index != ~0ULL;        // Localizer(max_index) of dfb_localize: range unknown
+  // dfb_localize (any max_index): measured, never dropped, and the engine's own range is neither used nor learned
+  const bool restricted = standalone || max_index != ~0ULL;
   if (h->id_bits > 0 && !restricted) {
     begin_bit = 64 - 4 * ((h->id_bits + 3) / 4);
   } else if (!restricted && !need_host_U && !exact_range) {
@@ -452,7 +463,7 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
                                   h->l_skeys.as<unsigned long long>(), h->l_spay.p, h->l_tmp.p, h->l_tmp.bytes, d_val,
                                   L.keys.as<uint64_t>(),
                                   L.col_start.as<int>(), L.col_end.as<int>(), L.lidx.as<uint32_t>(),
-                                  L.occ_sorted.p, scal, h->tab.prog, s);
+                                  L.occ_sorted.p, scal, drop_prog, s);
     if (nl < 0) return h->fail(DFB_ERR_CUDA, "radix sort / scan of the GPU localizer failed (temporary storage)");
     h->launches += nl;
   }
@@ -500,8 +511,16 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
   }
   DFB_CUDA(h, cudaEventRecord(L.done, ls));
   DFB_CUDA(h, cudaStreamWaitEvent(h->stream, L.done, 0));
-  int rc = step_dev(h, nrows, nnz, d_off, L.lidx.as<uint32_t>(), d_val, d_lab, L.keys.as<uint64_t>(), U, d_cnt,
-                    is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols);
+  int rc = 0;
+  if (!dev_count_ok && nnz && U == 0) {
+    // the localizer dropped the batch (ids outside the sorted range): no step; the drop is reported in this step's
+    // Progress, in stream order.  (With the count on the device, step_dev's kernels see the 0 and do the same.)
+    DFB_TRY(h->ensure(h->pred, nrows * sizeof(float)));       // what dfb_train_step_raw's pred_out copies
+    h->launches += launch_raise_err(h->tab.prog, kErrIdRange, h->stream);
+  } else {
+    rc = step_dev(h, nrows, nnz, d_off, L.lidx.as<uint32_t>(), d_val, d_lab, L.keys.as<uint64_t>(), U, d_cnt,
+                  is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols);
+  }
   DFB_CUDA(h, cudaEventRecord(L.consumed, h->stream));
   L.used = true;
   h->loc_seq++;
@@ -969,7 +988,7 @@ int dfb_auc(dfb_handle h, const float* label, const float* pred, size_t n, float
   DFB_TRY(h->ensure(h->cub, sort_tmp_bytes(n)));
   DFB_CUDA(h, cudaMemsetAsync(h->tab.prog + 1, 0, sizeof(DevProgress), s));
   h->launches += launch_auc(h->a_lab.as<float>(), h->a_pred.as<float>(), n, h->auc_k.as<float>(),
-                            h->auc_v.as<float>(), h->cub.p, h->cub.bytes, &(h->tab.prog + 1)->auc, s);
+                            h->auc_v.as<float>(), h->cub.p, h->cub.bytes, &(h->tab.prog + 1)->auc, nullptr, s);
   DevProgress pr;
   DFB_TRY(fetch_scratch(h, &pr));
   *auc_times_n = (float)pr.auc;
@@ -1144,7 +1163,8 @@ int dfb_localize(dfb_handle h, size_t nrows, const uint64_t* offset, const uint6
   size_t U = 0;
   DFB_CUDA(h, cudaStreamSynchronize(h->loc_stream));
   dfb_engine::LocSet& L = h->loc[0];
-  DFB_TRY(localize_dev(h, nrows, nnz, h->a_off.as<uint64_t>(), h->keys.as<uint64_t>(), nullptr, max_index, L, s, true, true, &U));
+  DFB_TRY(localize_dev(h, nrows, nnz, h->a_off.as<uint64_t>(), h->keys.as<uint64_t>(), nullptr, max_index, L, s, true, true, &U,
+                         nullptr, true));
   DFB_CUDA(h, cudaMemcpyAsync(index_out, L.lidx.p, nnz * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
   DFB_CUDA(h, cudaMemcpyAsync(keys_out, L.keys.p, U * sizeof(uint64_t), cudaMemcpyDeviceToHost, s));
   if (cnt_out) {
@@ -1599,7 +1619,7 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
     DFB_TRY(h->ensure(h->auc_v, nrows * sizeof(float)));
     DFB_TRY(h->ensure(h->auc_tmp, sort_tmp_bytes(nrows)));
     h->launches += launch_auc(d_label, h->pred.as<float>(), nrows, h->auc_k.as<float>(),
-                              h->auc_v.as<float>(), h->auc_tmp.p, h->auc_tmp.bytes, &h->tab.prog->auc, s);
+                              h->auc_v.as<float>(), h->auc_tmp.p, h->auc_tmp.bytes, &h->tab.prog->auc, nullptr, s);
   }
   // the worker evaluates the penalty of what it pulled (sgd_learner.cc:148)
   if (!sorted) h->launches += launch_penalty(h->prm, h->tab.prog, d_w, d_hasv, d_V, ks, 1, nkeys, nullptr, s);

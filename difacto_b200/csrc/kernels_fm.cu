@@ -58,6 +58,14 @@ __device__ __forceinline__ float row_p(float label, float pred) {
   return -y / (1.f + expf(y * pred));
 }
 
+// true when the GPU localizer dropped this batch (FmBatch::dev_nkeys): its ranks index nothing, so the kernel must
+// return before it reads them.  Block-uniform.  raise: this kernel reports the drop (one per forward launch).
+__device__ __forceinline__ bool batch_dropped(const FmBatch& b, bool raise) {
+  if (b.dev_nkeys == nullptr || *b.dev_nkeys != 0ULL) return false;
+  if (raise && blockIdx.x == 0 && threadIdx.x == 0 && b.prog) raise_err(b.prog, kErrIdRange);
+  return true;
+}
+
 __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, DevProgress* prog) {
   __shared__ float red_s[32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -99,6 +107,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
   constexpr int G = 32 / LPR;                // V rows fetched by one warp-wide load
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;   // independent loads in flight per lane
   constexpr bool PF = K <= DFB_FM_PF_MAXK;
+  if (MODE != 3 && batch_dropped(b, true)) return;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPR, grp = lane / LPR;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -274,6 +283,7 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;
   __shared__ float4 s_xv[kLongWarps][LPR];
   __shared__ float2 s_sc[kLongWarps];
+  if (batch_dropped(b, false)) return;                // k_fm_fast reports it
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
   const uint64_t pol_v = l2_policy(v.l2hint ? kL2EvictFirst : kL2Normal);
@@ -396,6 +406,7 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
 template <bool TRAIN>
 __global__ void __launch_bounds__(128) k_fm_generic(FmBatch b, FmView v) {
   extern __shared__ float smem[];
+  if (batch_dropped(b, true)) return;
   const int k = b.V_dim;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   float* xv = smem + (size_t)wid * k;

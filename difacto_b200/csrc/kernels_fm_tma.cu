@@ -61,6 +61,10 @@ __global__ void __launch_bounds__(kTmaWarps * 32) k_fm_tma(FmBatch b, FmView v) 
   constexpr int ROWB = K * 4;
   constexpr int STAGEB = 32 * ROWB;
   extern __shared__ __align__(128) unsigned char smem[];
+  if (b.dev_nkeys && *b.dev_nkeys == 0ULL) {          // dropped by the GPU localizer: see FmBatch::dev_nkeys
+    if (blockIdx.x == 0 && threadIdx.x == 0 && b.prog) atomicCAS(&b.prog->err, 0, kErrIdRange);
+    return;
+  }
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
   unsigned char* stage0 = smem + (size_t)wid * 2 * STAGEB;

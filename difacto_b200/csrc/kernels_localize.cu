@@ -170,11 +170,12 @@ k_emit(const KT* __restrict__ skeys, const Payload<KT>* __restrict__ spay, const
       col_start[r + 1] = (int)n;      // col_start doubles as the U+1 column offsets of the CSC view
       // scal = {OR of all keys, number of unique keys}.  A key bit below the sorted range means the range was
       // assumed too narrow (id_bits / the range learned from earlier batches): the batch is NOT sorted, so it is
-      // dropped (zero keys) and the error is reported instead of training on garbage.
+      // dropped (zero keys).  The single-GPU step sees the zero and reports the drop in stream order (prog ==
+      // nullptr here: this kernel runs on the localizer's stream, concurrently with the previous step's Progress).
       const unsigned long long low = begin_bit > 0 ? (scal[0] & ((1ULL << begin_bit) - 1ULL)) : 0ULL;
       if (low != 0ULL) {
         scal[1] = 0ULL;
-        if (prog) raise_err(prog, DFB_ERR_INVALID);
+        if (prog) raise_err(prog, kErrIdRange);
       } else {
         scal[1] = (unsigned long long)(r + 1);
       }
@@ -261,6 +262,13 @@ int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_
     passes = (64 - begin_bit + 7) / 8;
   }
   return 3 + passes;
+}
+
+__global__ void k_raise_err(DevProgress* prog, int code) { raise_err(prog, code); }
+
+int launch_raise_err(DevProgress* prog, int code, cudaStream_t s) {
+  k_raise_err<<<1, 1, 0, s>>>(prog, code);
+  return 1;
 }
 
 int launch_cnt_from_cols(const int* col_start, const int* col_end, size_t n, float* cnt, cudaStream_t s) {

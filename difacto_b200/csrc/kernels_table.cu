@@ -574,7 +574,9 @@ __global__ void k_evaluate(const float* __restrict__ label, const float* __restr
 }
 
 // BinClassMetric::AUC (bin_class_metric.h:35-56) on (pred ascending, label) pairs
-__global__ void __launch_bounds__(1024) k_auc_area(const float* __restrict__ sorted_label, size_t n, double* out_add) {
+__global__ void __launch_bounds__(1024) k_auc_area(const float* __restrict__ sorted_label, size_t n, double* out_add,
+                                                   const unsigned long long* __restrict__ dev_nkeys) {
+  if (dev_nkeys && *dev_nkeys == 0ULL) return;     // a batch the GPU localizer dropped: no prediction was made
   __shared__ unsigned long long s_tp[1024];
   __shared__ unsigned long long s_area[1024];
   const int tid = threadIdx.x;
@@ -1256,12 +1258,12 @@ int launch_evaluate(const float* label, const float* pred, size_t n, double* out
 }
 
 int launch_auc(const float* label, const float* pred, size_t n, float* key_tmp2, float* val_tmp2, void* cub_tmp,
-               size_t cub_bytes, double* out_add, cudaStream_t s) {
+               size_t cub_bytes, double* out_add, const unsigned long long* dev_nkeys, cudaStream_t s) {
   if (n == 0) return 0;
   // stable ascending radix sort by pred: ties keep original row order
   if (cub::DeviceRadixSort::SortPairs(cub_tmp, cub_bytes, pred, key_tmp2, label, val_tmp2, (int)n, 0, 32, s) != cudaSuccess)
     return -1;
-  k_auc_area<<<1, 1024, 0, s>>>(val_tmp2, n, out_add);
+  k_auc_area<<<1, 1024, 0, s>>>(val_tmp2, n, out_add, dev_nkeys);
   return 4;
 }
 

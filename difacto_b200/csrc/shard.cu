@@ -146,7 +146,7 @@ int shard_phase(dfb_engine* h, int phase) {
   DFB_TRY(h->ensure(sh.pred[d], (nrows ? nrows : 1) * sizeof(float)));
   {
     StageTimer tm(h, 5, W);
-    DFB_TRY(dfbh::localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, sh.L, W, false, false, &Ucap));   // Localizer(-1), sgd_learner.cc:203
+    DFB_TRY(dfbh::localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, sh.L, W, false, false, &Ucap, h->tab.prog));   // Localizer(-1), sgd_learner.cc:203
   }
   DFB_DBG(h, "localize");
   StageTimer tm_slice(h, 6, W);
@@ -291,7 +291,7 @@ int shard_phase(dfb_engine* h, int phase) {
     DFB_TRY(h->ensure(h->auc_tmp, sort_tmp_bytes(nrows)));
     DFB_CUDA(h, cudaStreamWaitEvent(A, sh.ev_reduce[d], 0));
     h->launches += launch_auc(d_lab, sh.pred[d].as<float>(), nrows, h->auc_k.as<float>(), h->auc_v.as<float>(),
-                              h->auc_tmp.p, h->auc_tmp.bytes, &sh.prog_w(d)->auc, A);
+                              h->auc_tmp.p, h->auc_tmp.bytes, &sh.prog_w(d)->auc, nullptr, A);
     DFB_CUDA(h, cudaEventRecord(sh.ev_auc[d], A));
   }
   }

@@ -79,9 +79,16 @@ typedef struct {
  *                         update keeps the per-row p*XV / p evict_last, streams the V rows evict_first and drops
  *                         p*XV / p from L2 afterwards
  *   id_bits (0)           > 0: feature ids are < 2^id_bits; fixes the bit range the GPU localizer's radix sort
- *                         visits.  0: the range is learned from the first raw batch (one 8-byte sync) and
- *                         verified on the device afterwards; a later batch with wider ids is dropped with
- *                         DFB_ERR_INVALID (pass id_bits, or use the synchronous dfb_train_step_raw)
+ *                         visits.  The range is rounded up to whole nibbles: ids below 2^(4*ceil(id_bits/4)) are
+ *                         accepted and sorted correctly.  0: the range is learned from the first raw batch (one
+ *                         8-byte sync) and verified on the device afterwards; it widens to a wider batch for the
+ *                         batches localized after that batch's key mask is read back (without waiting; at the
+ *                         latest after dfb_sync).  The synchronous dfb_train_step_raw of an engine without id_bits
+ *                         measures every batch.
+ *                         A raw batch with an id outside the range is DROPPED: it changes nothing (table, V rows,
+ *                         AdaGrad state, the InitV random stream), adds nothing to any Progress field, and the read
+ *                         of its Progress (dfb_train_step_raw, dfb_wait_step, dfb_read_progress) returns
+ *                         DFB_ERR_INVALID once, with a message naming the range.  dfb_localize ignores id_bits.
  *   shard_timeout_ms (20000)  how long a rank of the sharded store waits for a peer
  *   hot_split (256)       a key with more occurrences in a minibatch than this has its gradient pre-reduced in
  *                         chunks by separate warps, then finished in chunk order (0: one warp per key)
@@ -189,6 +196,7 @@ int dfb_train_step_async(dfb_handle h, size_t nrows, const uint64_t* offset,
 /* ---------------------------------------------------------------------------------
  * raw (un-localized) minibatches: Localizer::Compact on the device (SURVEY.md 8f rank 1).
  * dfb_localize is Localizer(max_index).Compact (src/data/localizer.h:41-51, localizer.cc:11-103)
+ * for any input (it measures the id range of every call: neither id_bits nor the learned range apply)
  * with host buffers in and out, bit-exact: index_out[nnz] = rank of every nnz's key, keys_out =
  * ascending unique ReverseBytes(id % max_index), cnt_out = occurrence counts (may be NULL).
  * dfb_train_step_raw* take the CSR<uint64> block the reader produced (BatchReader::Value) and run
