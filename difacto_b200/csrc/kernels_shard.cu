@@ -84,7 +84,9 @@ __global__ void k_shard_bounds(const uint64_t* __restrict__ keys, const unsigned
   b.kb[0] = 0;
   b.kb[S] = (int)U;
   for (int s = 0; s <= S; ++s) b.nb[s] = (U == 0) ? 0 : ((size_t)b.kb[s] < U ? col_start[b.kb[s]] : (int)nnz);
-  b.valid = U > 0 ? 1 : 0;
+  // no keys for non-zeros: the localizer dropped the batch (ids outside the sorted range) and reported it.  A batch
+  // without non-zeros is not dropped: its rows still count, with the bias-free prediction 0.
+  b.valid = (U > 0 || nnz == 0) ? 1 : 0;
   for (int s = 0; s < S; ++s)
     if ((size_t)(b.kb[s + 1] - b.kb[s]) > Kseg || (size_t)(b.nb[s + 1] - b.nb[s]) > Nseg) {
       // a key segment larger than the mailbox slot (skewed key distribution): drop the batch, report
@@ -274,6 +276,9 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
   __shared__ float red_s[8];
+  // a dropped batch: the owners sent no partials (their slots hold an older step's), so nothing is predicted, stored
+  // or added to Progress
+  if (!a.wb->valid) return;
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;

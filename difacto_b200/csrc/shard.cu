@@ -42,7 +42,7 @@ struct ShardState {
               ev_lookup[2] = {};
   uint64_t step = 0;
   dfb_engine::LocSet L;
-  DevBuf wb, rowcnt, pred[2];
+  DevBuf wb, rowcnt, pred[2];    // wb: ShardBounds [2] by step parity (the AUC of step t reads it beside step t+1)
   DevBuf slot[2], conf[2];        // by step parity: the lookup of step t+1 runs beside the update of step t
   DevBuf w, vrow, wv, vsave, flags, ws;
   DevProgress* dprog = nullptr;   // device: [0,S) per-worker scratch, [S,S+2) worker Progress by parity, [S+2,S+4) staging
@@ -64,6 +64,7 @@ struct ShardState {
   DevProgress* src_prog(int r) { return dprog + r; }
   DevProgress* prog_w(int d) { return dprog + S + d; }
   DevProgress* stage(int d) { return dprog + S + 2 + d; }
+  ShardBounds* bounds(int d) { return wb.as<ShardBounds>() + d; }
 };
 
 namespace {
@@ -146,13 +147,15 @@ int shard_phase(dfb_engine* h, int phase) {
   DFB_TRY(h->ensure(sh.pred[d], (nrows ? nrows : 1) * sizeof(float)));
   {
     StageTimer tm(h, 5, W);
-    DFB_TRY(dfbh::localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, sh.L, W, false, false, &Ucap, h->tab.prog));   // Localizer(-1), sgd_learner.cc:203
+    // a dropped batch (range, or a segment over its capacity below) is reported into this step's own Progress slot:
+    // the engine-wide one may still be read by the previous step's snapshot, which runs beside this stream
+    DFB_TRY(dfbh::localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, sh.L, W, false, false, &Ucap, sh.prog_w(d)));   // Localizer(-1), sgd_learner.cc:203
   }
   DFB_DBG(h, "localize");
   StageTimer tm_slice(h, 6, W);
-  ShardBounds* wb = sh.wb.as<ShardBounds>();
+  ShardBounds* wb = sh.bounds(d);
   h->launches += launch_shard_bounds(sh.L.keys.as<uint64_t>(), sh.L.dU(), Ucap, sh.L.col_start.as<int>(), nnz, S, Kseg,
-                                     lay.Nseg, wb, h->tab.prog, W);
+                                     lay.Nseg, wb, sh.prog_w(d), W);
   {
     ScatterArgs a;
     memset(&a, 0, sizeof(a));
@@ -264,7 +267,7 @@ int shard_phase(dfb_engine* h, int phase) {
     StageTimer tm_red(h, 8, W);
     ReduceArgs ra;
     memset(&ra, 0, sizeof(ra));
-    ra.S = S; ra.me = me; ra.train = is_train ? 1 : 0; ra.nrows = nrows;
+    ra.S = S; ra.me = me; ra.train = is_train ? 1 : 0; ra.nrows = nrows; ra.wb = sh.bounds(d);
     for (int s = 0; s < S; ++s) {
       ra.part_xv[s] = lay.at<float>(mine, lay.off_part_xv, lay.str_part_xv, d, s);
       ra.part_sc[s] = lay.at<float2>(mine, lay.off_part_sc, lay.str_part_sc, d, s);
@@ -290,8 +293,9 @@ int shard_phase(dfb_engine* h, int phase) {
     DFB_TRY(h->ensure(h->auc_v, nrows * sizeof(float)));
     DFB_TRY(h->ensure(h->auc_tmp, sort_tmp_bytes(nrows)));
     DFB_CUDA(h, cudaStreamWaitEvent(A, sh.ev_reduce[d], 0));
+    // a dropped batch made no prediction: ShardBounds::valid == 0 makes the AUC add nothing
     h->launches += launch_auc(d_lab, sh.pred[d].as<float>(), nrows, h->auc_k.as<float>(), h->auc_v.as<float>(),
-                              h->auc_tmp.p, h->auc_tmp.bytes, &sh.prog_w(d)->auc, nullptr, A);
+                              h->auc_tmp.p, h->auc_tmp.bytes, &sh.prog_w(d)->auc, &sh.bounds(d)->valid, A);
     DFB_CUDA(h, cudaEventRecord(sh.ev_auc[d], A));
   }
   }
@@ -454,7 +458,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
       if ((e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
   const size_t tot = (size_t)nranks * Kseg;
   int rc = 0;
-  if ((rc = h->ensure(sh->wb, sizeof(ShardBounds))) || (rc = h->ensure(sh->slot[0], tot * 4)) || (rc = h->ensure(sh->slot[1], tot * 4)) || (rc = h->ensure(sh->w, tot * 4)) ||
+  if ((rc = h->ensure(sh->wb, 2 * sizeof(ShardBounds))) || (rc = h->ensure(sh->slot[0], tot * 4)) || (rc = h->ensure(sh->slot[1], tot * 4)) || (rc = h->ensure(sh->w, tot * 4)) ||
       (rc = h->ensure(sh->vrow, tot * 4)) || (rc = h->ensure(sh->wv, tot * 8)) || (rc = h->ensure(sh->flags, tot * 4)) ||
       (rc = h->ensure(sh->ws, (tot / 32 + 64) * 4)))
     return fail(rc);

@@ -25,8 +25,9 @@ namespace dfb {
 struct ShardBounds {
   int kb[9];     // key index boundaries of the owners' segments in the worker's sorted key list
   int nb[9];     // the same boundaries in the CSC payload (non-zeros)
-  int valid;     // 0: the batch is dropped (error raised): every segment is sent empty
-  int pad;
+  // 0: the batch is dropped (error raised into the step's Progress): every segment is sent empty, and the worker's
+  // reduce and AUC add nothing.  A u64, so that k_auc_area can take it as its "dropped when 0" count.
+  unsigned long long valid;
 };
 
 struct ShardLayout {
@@ -87,6 +88,7 @@ struct FillDst { uint32_t* ridx_dst[8]; float* rval_dst[8]; };
 struct ReduceArgs {
   int S, me, train;
   size_t nrows;
+  const ShardBounds* wb;       // !wb->valid: the batch was dropped, the owners computed no partials for it
   const float* part_xv[8];
   const float2* part_sc[8];
   float* p_dst[8];

@@ -337,6 +337,11 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
  * Results: dfb_wait_step (per step) / dfb_read_progress (accumulated), as for the other async entry points;
  * Progress is this rank's own minibatch (loss, AUC, penalty of the weights it used).  DFB_ERR_TIMEOUT: a peer
  * did not reach the step within shard_timeout_ms (kwarg, default 20000).
+ * A dropped batch: a rank's batch with an id outside the id range (id_bits, or the range learned from earlier
+ * batches), or with a key segment larger than seg_keys / seg_nnz, changes nothing on any owner and adds nothing
+ * to that rank's loss, penalty, AUC or row count (its new_keys / new_vrows count what this rank inserted as an
+ * owner, for the other workers); the other ranks step as if it held an empty batch.  It is reported once,
+ * by that rank's read of its own step: DFB_ERR_INVALID (range) or DFB_ERR_CAPACITY (segment).
  * ------------------------------------------------------------------------------- */
 int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t max_nnz, size_t seg_keys,
                    size_t seg_nnz, size_t* mailbox_bytes_out);

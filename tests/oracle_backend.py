@@ -29,17 +29,18 @@ class OracleBackend:
 
     def pull_rows(self, keys, w, hasv, V):
         k = self.V_dim
+        if not len(keys):
+            return
+        n = len(keys)
         vals, lens = self.M.get(_keys_np(keys))
-        p = 0
-        for i in range(len(keys)):
-            w[i] = float(vals[p])
-            p += 1
-            if k and lens[i] > 1:
-                V[i, :k] = torch.from_numpy(vals[p:p + k].copy())
-                hasv[i] = 1
-                p += k
-            else:
-                hasv[i] = -1
+        if not k:                                   # V_dim 0: one value per key, no lens
+            lens = np.ones(n, np.int32)
+        start = np.cumsum(lens) - lens
+        w[:n] = torch.from_numpy(vals[start])
+        has = lens > 1
+        hasv[:n] = torch.from_numpy(np.where(has, 1, -1).astype(np.int32))
+        if has.any():
+            V[torch.from_numpy(np.nonzero(has)[0]), :k] = torch.from_numpy(vals[start[has, None] + 1 + np.arange(k)])
 
     def _ragged(self, w, hasv, V):
         k = self.V_dim
@@ -50,9 +51,8 @@ class OracleBackend:
         w_pos, V_pos = O.get_pos(lens)
         vals = np.zeros(int(lens.sum()), np.float32)
         vals[w_pos] = w.numpy()
-        for i in range(U):
-            if V_pos[i] >= 0:
-                vals[V_pos[i]:V_pos[i] + k] = V[i, :k].numpy()
+        m = V_pos >= 0
+        vals[V_pos[m, None] + np.arange(k)] = V[:U, :k].numpy()[m]
         return vals, w_pos, V_pos, lens
 
     def fm_step(self, batch, w, hasv, V, is_train, gw, gV):
@@ -74,9 +74,8 @@ class OracleBackend:
             gw[:] = torch.from_numpy(g)
             return
         gw[:] = torch.from_numpy(g[w_pos])
-        for i in range(batch["U"]):
-            if V_pos[i] >= 0:
-                gV[i, :k] = torch.from_numpy(g[V_pos[i]:V_pos[i] + k].copy())
+        m = np.nonzero(V_pos >= 0)[0]
+        gV[torch.from_numpy(m), :k] = torch.from_numpy(g[V_pos[m, None] + np.arange(k)])
 
     def push_rows(self, keys, gw, hasv, gV):
         if not len(keys):
@@ -89,7 +88,6 @@ class OracleBackend:
         w_pos, V_pos = O.get_pos(lens)
         g = np.zeros(int(lens.sum()), np.float32)
         g[w_pos] = gw.numpy()
-        for i in range(len(keys)):
-            if V_pos[i] >= 0:
-                g[V_pos[i]:V_pos[i] + k] = gV[i, :k].numpy()
+        m = V_pos >= 0
+        g[V_pos[m, None] + np.arange(k)] = gV[:, :k].numpy()[m]
         self.M.update_grad(_keys_np(keys), g, lens)

@@ -8,6 +8,7 @@ on oracle shards (tests/shard_sim.py).  The protocol is exercised
   * with one process per GPU over CUDA IPC when 2 GPUs are visible.
 Tolerances as in test_gpu_parity.py: model state after T steps rel 1e-3 / abs 1e-5 (fp32, different summation
 order over k and over the owners' partials); keys, has-V flags, feature counts bit-exact."""
+import ctypes as C
 import os
 import socket
 import sys
@@ -22,63 +23,20 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 
-from shard_sim import all_keys, key_owner_np, raw_batch, simulate  # noqa: E402
+from oracle import oracle as O  # noqa: E402
+from shard_sim import (STATE_TOL, all_keys, check_progress, check_shard, check_vs_simulation, enqueue_local,  # noqa: E402
+                       key_owner_np, make_local, raw_batch, run_local, simulate)
 from util import assert_close, oracle_state  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 capi = pytest.importorskip("difacto_b200.capi")
 
-STATE_TOL = dict(rtol=1e-3, atol=1e-5)
 KW = dict(V_dim=16, l1=0.05, l2=0.01, lr=0.2, V_lr=0.1, V_threshold=1, V_l2=0.01, V_init_scale=0.2, seed=3)
 STEPS = 6
 
 
 def batch_fn(rank, step):
     return raw_batch(rank, step, valued=(step % 2 == 0))
-
-
-def check_shard(E, shard, keys, what):
-    scal, hasv, V, cg = E.read_entries(keys)
-    oscal, ohasv, oV, ocg = oracle_state(shard.M, keys)
-    assert np.array_equal(hasv, ohasv), what
-    assert np.array_equal(scal[:, 0], oscal[:, 0]), what                     # feature counts: exact
-    assert_close(scal[:, 1:], oscal[:, 1:], what=f"{what} w/sqrt_g/z", **STATE_TOL)
-    assert_close(V, oV, what=f"{what} V", **STATE_TOL)
-    assert_close(cg, ocg, what=f"{what} cg", **STATE_TOL)
-    assert E.table_stats()["n_keys"] == shard.M.size(), what
-
-
-def check_progress(pr, ref, what):
-    # ref = [loss, penalty, auc, nnz_w, nrows]
-    assert abs(pr.loss - ref[0]) <= 1e-4 * abs(ref[0]) + 1e-4, (what, pr.loss, ref[0])
-    assert abs(pr.penalty - ref[1]) <= 1e-4 * abs(ref[1]) + 1e-5, (what, pr.penalty, ref[1])
-    # AUC * n: predictions that are tied in exact arithmetic (rows whose only active feature is the same) are
-    # ordered by rounding; each flipped pair moves AUC * n by n / (n_pos * n_neg) <= ~0.05 at these sizes
-    if ref[4] > 0:     # (the reference never evaluates an empty batch; a worker without one contributes nothing)
-        assert abs(pr.auc - ref[2]) <= 1e-4 * abs(ref[2]) + 0.3, (what, pr.auc, ref[2])
-    assert pr.nrows == ref[4], (what, pr.nrows, ref[4])
-
-
-def run_local(S, kw, steps, fn, train_fn=None, devices=None, **shard_kw):
-    from difacto_b200.sharded import FusedShardedStore
-    engines = [capi.Engine(device=devices[r] if devices else 0, table_capacity=1 << 14, shard_timeout_ms=8000, **kw)
-               for r in range(S)]
-    shard_kw.setdefault("max_rows", 128)
-    shard_kw.setdefault("max_nnz", 4096)
-    FusedShardedStore.connect_local(engines, **shard_kw)
-    prog = [[] for _ in range(S)]
-    for step in range(steps):
-        is_train = True if train_fn is None else train_fn(step)
-        # one host thread, several engines on one device: interleave the five enqueue phases (see difacto_b200.h)
-        for r in range(S):
-            off, idx, val, lab = fn(r, step)
-            engines[r].shard_begin_async(len(lab), off, idx, val, lab, push_cnt=step < 2, is_train=is_train)
-        for phase in range(5):
-            for r in range(S):
-                engines[r].shard_phase(phase)
-        for r in range(S):
-            prog[r].append(engines[r].wait_step())
-    return engines, prog
 
 
 @pytest.mark.parametrize("S", [1, 2, 3])
@@ -177,20 +135,130 @@ def test_fused_shard_mixed_binary_valued_and_empty_batches():
         E.close()
 
 
+# ---------------------------------------------------------------------------------------------------------
+# dropped worker batches: nothing changes on any owner, nothing is added to that rank's Progress, and the error is
+# reported once, by that rank's read of its own step.  The other ranks step as if the worker held an empty batch.
+# (new_keys / new_vrows of a rank count its inserts as an OWNER, for every worker's keys: not the dropped batch's.)
+# ---------------------------------------------------------------------------------------------------------
+PROGRESS = ("loss", "penalty", "auc", "nrows", "new_keys", "new_vrows")
+WORKER = ("loss", "penalty", "auc", "nrows")
+ZERO = (0.0,) * 4 + (0, 0)
+
+
+def run_pipelined(engines, fn, steps):
+    """step t + 1 is enqueued before step t is read.  Returns per rank and step (rc, Progress, error message)"""
+    out = [[] for _ in engines]
+
+    def read(t):
+        for r, E in enumerate(engines):
+            pr = capi.Progress()
+            rc = E.L.dfb_wait_step(E.h, C.byref(pr))
+            out[r].append((rc, pr, E.L.dfb_last_error(E.h).decode() if rc else ""))
+    for t in range(steps):
+        enqueue_local(engines, [fn(r, t) for r in range(len(engines))], t < 2, True)
+        if t:
+            read(t - 1)
+    read(steps - 1)
+    for E in engines:
+        E.sync()
+        assert tuple(getattr(E.read_progress(), f) for f in PROGRESS) == ZERO       # nothing left behind
+    return out
+
+
+def check_dropped(engines, out, kw, steps, fn, fn_sim, bad, code, what):
+    """out of run_pipelined; bad = (rank, step) of the dropped batch, code its error.  Returns the error message"""
+    S = len(engines)
+    prog = [[pr for _, pr, _ in o] for o in out]
+    msg = None
+    for r in range(S):
+        for t in range(steps):
+            rc, pr, m = out[r][t]
+            if (r, t) == bad:
+                assert rc == code, f"{what}: rank {r} step {t}: rc {rc} ({m})"
+                assert tuple(getattr(pr, f) for f in WORKER) == ZERO[:4], f"{what}: Progress of the dropped batch"
+                msg = m
+            else:
+                assert rc == 0, f"{what}: rank {r} step {t}: rc {rc} ({m})"
+    check_vs_simulation(engines, prog, kw, steps, fn_sim, what)
+    own_keys = all_keys(S, steps, fn_sim)
+    dropped_only = np.setdiff1d(O.localize(*fn(*bad)[:2])[1], own_keys)
+    assert len(dropped_only)
+    for E in engines:
+        assert np.all(E.read_entries(dropped_only)[1] == -1), f"{what}: a key of the dropped batch was inserted"
+    return msg
+
+
+def rand_ids(rng, n, bits):
+    x = (rng.integers(0, 1 << 32, n, dtype=np.uint64) << np.uint64(32)) | rng.integers(0, 1 << 32, n, dtype=np.uint64)
+    return x & np.uint64((1 << bits) - 1)
+
+
+@pytest.mark.parametrize("S", [2, 3])
+@pytest.mark.parametrize("id_bits", [16, 30, 36, None])
+def test_fused_shard_batch_outside_id_range_is_dropped(id_bits, S):
+    """id_bits 16 / 30 (32-bit sort keys), 36 (64-bit), None (the range learned from the first batch: ids below 2^12).
+    Rank 1's batch of step 2 carries one id above the range (id_bits: 2^nibble_top, the smallest id outside it;
+    learned: ids of 40 bits)"""
+    bits = id_bits or 12
+    top = 4 * ((bits + 3) // 4)
+    pool = np.unique(rand_ids(np.random.default_rng(bits), 3000, bits))
+    steps, bad = 5, (1, 2)
+
+    def legal(rank, step):
+        rng = np.random.default_rng(10 * rank + step + 100 * bits)
+        lens = rng.integers(0, 30, 120)
+        off = np.concatenate([[0], np.cumsum(lens)]).astype(np.uint64)
+        idx = pool[rng.integers(0, len(pool), int(off[-1]))]
+        val = rng.random(len(idx)).astype(np.float32) if (rank + step) % 2 else None
+        lab = np.where(rng.random(120) < 0.4, 1.0, -1.0).astype(np.float32)
+        return off, idx, val, lab
+
+    def fn(rank, step):
+        off, idx, val, lab = legal(rank, step)
+        if (rank, step) != bad:
+            return off, idx, val, lab
+        idx = idx.copy()
+        if id_bits:
+            idx[-1] = np.uint64(1 << top)
+        else:
+            idx[::3] = rand_ids(np.random.default_rng(7), len(idx[::3]), 40) | np.uint64(1 << 39)
+        return off, idx, val, lab
+
+    def fn_sim(rank, step):
+        return raw_batch(rank, step, valued=False, B=0) if (rank, step) == bad else fn(rank, step)
+    kw = dict(KW, V_dim=32)
+    engines = make_local(S, kw, engine_kw=dict(id_bits=id_bits) if id_bits else None, max_nnz=8192)
+    out = run_pipelined(engines, fn, steps)
+    msg = check_dropped(engines, out, kw, steps, fn, fn_sim, bad, capi.DFB_ERR_INVALID, f"id_bits={id_bits} S={S}")
+    assert "id_bits = %d" % (id_bits or 0) in msg, msg
+    if id_bits:
+        assert "2^%d" % top in msg, msg
+
+
 def test_fused_shard_segment_capacity_is_reported():
-    from difacto_b200.sharded import FusedShardedStore
-    engines = [capi.Engine(device=0, table_capacity=1 << 14, shard_timeout_ms=8000, **KW) for _ in range(2)]
-    FusedShardedStore.connect_local(engines, max_rows=128, max_nnz=4096, seg_keys=8, seg_nnz=16)
-    for r in range(2):
-        off, idx, val, lab = batch_fn(r, 0)
-        engines[r].shard_begin_async(len(lab), off, idx, val, lab, push_cnt=False, is_train=True)
-    for phase in range(5):
-        for r in range(2):
-            engines[r].shard_phase(phase)
-    with pytest.raises(capi.DfbError) as ei:
-        for r in range(2):
-            engines[r].wait_step()
-    assert ei.value.code == capi.DFB_ERR_CAPACITY
+    """a key segment larger than seg_keys on rank 1 in step 2 of 4 drops that batch alone, reported with its step"""
+    steps, bad = 4, (1, 2)
+
+    def fn(rank, step):     # 60 ids: at most 60 keys per owner segment; the bad batch has ~500 over 2 owners
+        return raw_batch(rank, step, valued=step % 2 == 0, ids=500 if (rank, step) == bad else 60)
+
+    def fn_sim(rank, step):
+        return raw_batch(rank, step, valued=False, B=0) if (rank, step) == bad else fn(rank, step)
+    engines = make_local(2, KW, max_rows=128, max_nnz=4096, seg_keys=64, seg_nnz=2048)
+    out = run_pipelined(engines, fn, steps)
+    check_dropped(engines, out, KW, steps, fn, fn_sim, bad, capi.DFB_ERR_CAPACITY, "segment capacity")
+
+
+def test_fused_shard_rows_without_nonzeros_count():
+    """a worker batch with rows but no nonzeros is not dropped: its rows count, with prediction 0"""
+    def fn(rank, step):
+        if rank == 1 and step in (1, 2):
+            off, idx, val, lab = raw_batch(rank, step, valued=step == 2, B=40)
+            return np.zeros_like(off), idx[:0], None if val is None else val[:0], lab
+        return batch_fn(rank, step)
+    engines, prog = run_local(2, KW, 4, fn)
+    check_vs_simulation(engines, prog, KW, 4, fn, "rows without nonzeros")
+    assert prog[1][1].nrows == 40 and prog[1][2].nrows == 40
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
