@@ -191,9 +191,6 @@ size_t l2_bytes();
 // ---- launchers (kernels_fm.cu) ----
 // returns number of kernel launches performed, or <0 on invalid configuration
 int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s);
-// the bulk-copy (cp.async.bulk / UBLKCP) variant of the predict kernel for V_dim = 64 (kernels_fm_tma.cu, an A/B);
-// returns 0 when the configuration is outside the experiment
-int launch_fm_tma_predict(const FmBatch& b, const FmView& v, cudaStream_t s);
 // MODE 3: partial interaction sums of every source's rows (see PartArgs); v.vbase/vstride = the table rows
 int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s);
 int launch_grad_finalize(int V_dim, size_t nkeys, const float* weights, const int* V_pos,
@@ -203,7 +200,6 @@ int launch_grad_finalize_dense(int V_dim, int ks, size_t nkeys, const int* hasv,
                                const float* xxp, float* gV, cudaStream_t s);
 
 // ---- launchers (kernels_table.cu) ----
-extern int g_lookup_ilp, g_lookup_ctas, g_update_persistent;
 int launch_table_init(Table& t, unsigned seed, cudaStream_t s);
 // find (or insert) keys; slot_out[i] = hash position or -1.  When pull outputs are non-null also
 // emits w and vrow of each entry.

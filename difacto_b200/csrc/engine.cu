@@ -225,7 +225,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   if (U > 0x7fffffffULL || nrows > 0x7fffffffULL || nnz > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "batch too large");
   if (is_train && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data");   // CHECK(has_aux_), sgd_updater.cc:75
-  const bool sorted = is_train && h->scatter_sorted && !h->force_generic && fm_fast_supported(h->prm.V_dim);
+  const bool sorted = is_train && h->sorted_path();
   const int ks = h->tab.ks;
   cudaStream_t s = h->stream;
   DFB_TRY(ensure_key_ws(h, U));
@@ -298,9 +298,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   }
   if (nrows) {
     StageTimer tm(h, 1);
-    int nl = 0;
-    if (h->k1_tma && !is_train && !h->force_generic) nl = launch_fm_tma_predict(b, v, s);
-    if (nl == 0) nl = launch_fm(b, v, h->force_generic, s);
+    const int nl = launch_fm(b, v, h->force_generic, s);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
     h->launches += nl;
   }
@@ -492,7 +490,7 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
   cudaStream_t ls = h->profile ? h->stream : h->loc_stream;
   if (inputs_ready) DFB_CUDA(h, cudaStreamWaitEvent(ls, inputs_ready, 0));
   if (L.used) DFB_CUDA(h, cudaStreamWaitEvent(ls, L.consumed, 0));
-  const bool dev_count_ok = !h->force_generic && fm_fast_supported(h->prm.V_dim) && (!is_train || h->scatter_sorted);
+  const bool dev_count_ok = h->sorted_path(is_train);
   size_t U = 0;
   if (h->profile && h->prof_steps && h->prof_steps % dfb_engine::kProfRing == 0) DFB_TRY(prof_drain(h));
   {
@@ -554,7 +552,6 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   p.l1 = 1.f; p.l2 = 0.f; p.V_l2 = .01f; p.lr = .01f; p.lr_beta = 1.f; p.V_lr = .01f; p.V_lr_beta = 1.f;
   p.V_init_scale = .01f; p.V_threshold = 10; p.V_dim = -1; p.seed = 0;
   long long table_capacity = 1 << 20, v_capacity = -1;
-  int l2_fetch = 0;
   struct FR { const char* name; float* dst; float lo, hi; };
   FR fr[] = {{"l1", &p.l1, 0, 1e10f}, {"l2", &p.l2, 0, 1e10f}, {"V_l2", &p.V_l2, 0, 1e10f},
              {"lr", &p.lr, 0, 10}, {"lr_beta", &p.lr_beta, 0, 1e10f}, {"V_lr", &p.V_lr, 0, 1e10f},
@@ -591,15 +588,7 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else if (k == "V_capacity") { if (!need_int(0, 1LL << 30)) { delete h; return DFB_ERR_PARAM; } v_capacity = x; }
     else if (k == "compute_auc") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->compute_auc = (int)x; }
     else if (k == "force_generic") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->force_generic = (int)x; }
-    else if (k == "l2_fetch_granularity") {
-      if (!need_int(32, 128)) { delete h; return DFB_ERR_PARAM; }
-      l2_fetch = (int)x;
-    }
     else if (k == "overlap_auc") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->overlap_auc = (int)x; }
-    else if (k == "lookup_ilp") { if (!need_int(1, 4)) { delete h; return DFB_ERR_PARAM; } g_lookup_ilp = (int)x; }
-    else if (k == "update_persistent") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } g_update_persistent = (int)x; }
-    else if (k == "lookup_ctas") { if (!need_int(1, 64)) { delete h; return DFB_ERR_PARAM; } g_lookup_ctas = (int)x; }
-    else if (k == "k1_tma") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->k1_tma = (int)x; }
     else if (k == "long_row_nnz") { if (!need_int(0, 1 << 30)) { delete h; return DFB_ERR_PARAM; } h->long_row_nnz = (int)x; }
     else if (k == "hot_split") { if (!need_int(0, 1 << 30)) { delete h; return DFB_ERR_PARAM; } h->hot_split = (int)x; }
     else if (k == "l2_hints") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->l2_hints = (int)x; }
@@ -624,7 +613,6 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     return (int)DFB_ERR_CUDA;
   };
   if ((e = cudaSetDevice(h->device)) != cudaSuccess) return cfail("cudaSetDevice");
-  if (l2_fetch) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)l2_fetch);   // a hint; errors ignored
   if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
   if ((e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
   if ((e = cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
@@ -1543,8 +1531,7 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
   for (int i = 0; i < nseg; ++i) { sd.gw[i] = peer_gw[i]; sd.gV[i] = peer_gV[i]; }
   if (first_seg >= 0 && first_seg < nseg) sd.rot = sd.bounds[first_seg] / 32 * 32;
   if ((size_t)sd.bounds[nseg] != nkeys) return h->fail(DFB_ERR_INVALID, "seg_bounds[nseg] must equal nkeys");
-  const int k = h->prm.V_dim;
-  if (!(h->scatter_sorted && !h->force_generic && fm_fast_supported(k) && h->tab.ks == k))
+  if (!h->sorted_path())
     return h->fail(DFB_ERR_INVALID, "peer gradient stores need the sorted scatter path (V_dim in {8,16,32,64,128})");
   return dev_fm_step_impl(h, nrows, nnz, d_offset, d_index, d_value, d_label, nkeys, d_w, d_hasv, d_V, 1,
                           peer_gw[0], peer_gV[0], &sd);
@@ -1560,7 +1547,7 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
   const int ks = h->tab.ks, k = h->prm.V_dim;
   if (nkeys > 0x7fffffffULL || nrows > 0x7fffffffULL || nnz > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "batch too large");
-  const bool sorted = is_train && h->scatter_sorted && !h->force_generic && fm_fast_supported(k) && ks == k;
+  const bool sorted = is_train && h->sorted_path();
   DFB_TRY(h->ensure(h->pred, nrows * sizeof(float)));
   FmView v;
   memset(&v, 0, sizeof(v));

@@ -30,7 +30,6 @@ struct dfb_engine {
   int id_bits = 0;          // > 0: feature ids are < 2^id_bits (fixes the radix-sort bit range of the GPU localizer)
   int loc_begin_bit = -1;   // auto mode: lowest significant bit of the reversed keys seen so far (sticky)
   long long shard_timeout_ms = 20000;
-  int k1_tma = 0;           // 1: validation batches use the bulk-copy staged gather kernel (kernels_fm_tma.cu)
   int long_row_nnz = 1024;  // rows with at least this many nonzeros are walked by a whole CTA (k_fm_long); 0: off
   int hot_split = 256;      // occurrence lists longer than this are pre-reduced in chunks by separate warps (0: off)
   cudaStream_t stream = nullptr, copy_stream = nullptr, aux_stream = nullptr;
@@ -95,6 +94,11 @@ struct dfb_engine {
   unsigned long long* h_nvals = nullptr;  // pinned
   ShardState* shard = nullptr;          // the NVLink-sharded store this engine is a rank of (shard.cu)
 
+  // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (V_dim in {8,16,32,64,128}) and,
+  // when it trains, the atomic-free sorted gradient reduction
+  bool sorted_path(bool is_train = true) const {
+    return !force_generic && dfb::fm_fast_supported(prm.V_dim) && (!is_train || scatter_sorted);
+  }
   int fail(int code, const std::string& msg) { err = msg; return code; }
   int cuda_fail(cudaError_t e, const char* what) {
     err = std::string(what) + ": " + cudaGetErrorString(e);

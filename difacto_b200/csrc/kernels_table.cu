@@ -46,33 +46,34 @@ __global__ void k_table_init(Entry* tab, uint64_t cap, TableState* st, DevProgre
 
 // model_[key] (sgd_updater.cc:43-45,65-67,86-88): find or default-construct, and the Pull of the
 // fused path (w and the V-row index of every key).  Random 32-byte sectors: the kernel is latency
-// bound, so every thread keeps ILP independent first probes in flight (both halves of the entry are
-// fetched with the probe; a hit needs no second round trip) and only collisions fall back to the
-// serial probe loop.
-template <bool INSERT, int ILP>
+// bound, so every thread keeps kLookupIlp = 2 independent first probes in flight (both halves of the
+// entry are fetched with the probe; a hit needs no second round trip) and only collisions fall back to
+// the serial probe loop.
+constexpr int kLookupIlp = 2;
+template <bool INSERT>
 __global__ void __launch_bounds__(256) k_lookup(Table t, const uint64_t* __restrict__ keys, size_t n_cap,
                                                 const unsigned long long* __restrict__ dn,
                                                 int* __restrict__ slot_out, float* __restrict__ w_out,
                                                 int* __restrict__ vrow_out, int2* __restrict__ wv_out) {
   const size_t n = dev_count(n_cap, dn);
-  const size_t tile = (size_t)blockDim.x * ILP;
+  const size_t tile = (size_t)blockDim.x * kLookupIlp;
   for (size_t base = (size_t)blockIdx.x * tile; base < n; base += (size_t)gridDim.x * tile) {
-    unsigned long long key[ILP];
-    uint64_t h[ILP];
-    Entry256 e[ILP];
+    unsigned long long key[kLookupIlp];
+    uint64_t h[kLookupIlp];
+    Entry256 e[kLookupIlp];
 #pragma unroll
-    for (int q = 0; q < ILP; ++q) {
+    for (int q = 0; q < kLookupIlp; ++q) {
       const size_t i = base + (size_t)q * blockDim.x + threadIdx.x;
       key[q] = i < n ? keys[i] : 0ULL;
       h[q] = hash64(key[q]) & t.mask;
     }
 #pragma unroll
-    for (int q = 0; q < ILP; ++q) {
+    for (int q = 0; q < kLookupIlp; ++q) {
       const size_t i = base + (size_t)q * blockDim.x + threadIdx.x;
       if (i < n) e[q] = load_entry(&t.tab[h[q]]);
     }
 #pragma unroll
-    for (int q = 0; q < ILP; ++q) {
+    for (int q = 0; q < kLookupIlp; ++q) {
       const size_t i = base + (size_t)q * blockDim.x + threadIdx.x;
       if (i >= n) continue;
       int slot = -1, vr = -1;
@@ -1131,9 +1132,6 @@ size_t l2_bytes() {
   return (size_t)cached_attr(cache, cudaDevAttrL2CacheSize, 50 << 20);
 }
 
-// tuning knobs of k_lookup (engine kwargs lookup_ilp / lookup_ctas; process-wide)
-int g_lookup_ilp = 2, g_lookup_ctas = 64, g_update_persistent = 0;
-
 int launch_table_init(Table& t, unsigned seed, cudaStream_t s) {
   k_table_init<<<num_sms() * 8, 256, 0, s>>>(t.tab, t.cap, t.state, t.prog, seed);
   return 1;
@@ -1142,15 +1140,9 @@ int launch_table_init(Table& t, unsigned seed, cudaStream_t s) {
 int launch_lookup(Table& t, const uint64_t* keys, size_t n, const unsigned long long* dn, bool insert,
                   int* slot_out, float* w_out, int* vrow_out, int2* wv_out, cudaStream_t s) {
   if (n == 0) return 0;
-  const int ilp = g_lookup_ilp;
-  const int grid = grid_for(n, 256 * ilp, num_sms() * g_lookup_ctas);
-#define DFB_LK(I)                                                                                            \
-  do {                                                                                                       \
-    if (insert) k_lookup<true, I><<<grid, 256, 0, s>>>(t, keys, n, dn, slot_out, w_out, vrow_out, wv_out);   \
-    else        k_lookup<false, I><<<grid, 256, 0, s>>>(t, keys, n, dn, slot_out, w_out, vrow_out, wv_out);  \
-  } while (0)
-  if (ilp == 1) DFB_LK(1); else if (ilp == 2) DFB_LK(2); else DFB_LK(4);
-#undef DFB_LK
+  const int grid = grid_for(n, 256 * kLookupIlp, num_sms() * 64);
+  if (insert) k_lookup<true><<<grid, 256, 0, s>>>(t, keys, n, dn, slot_out, w_out, vrow_out, wv_out);
+  else        k_lookup<false><<<grid, 256, 0, s>>>(t, keys, n, dn, slot_out, w_out, vrow_out, wv_out);
   return 1;
 }
 
@@ -1321,12 +1313,12 @@ int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pul
   k_bwd_update<K, VAL, true, SRC, HINT><<<grid, 256, 0, s>>>(t, p, slot, pull_vrow, n, dn, col_start, col_end,       \
                                                              occ_sorted, p_row, pxv, flags, acc_pen, nullptr, nullptr, \
                                                              nullptr, noseg, sa, hp)
+  // one short-lived CTA per 256 keys, so that the higher-priority streams working on the NEXT step (localizer;
+  // worker / lookup streams of the sharded store) get SM slots as CTAs retire -- a grid-stride grid holds every
+  // slot until the kernel ends
+  const int grid = grid_warps((n + 31) / 32, 8, 1 << 22);
 #define DFB_BU(K)                                                                                          \
   do {                                                                                                     \
-    /* one short-lived CTA per 256 keys, so that the higher-priority streams working on the NEXT step (localizer;  \
-       worker / lookup streams of the sharded store) get SM slots as CTAs retire -- a grid-stride grid holds     \
-       every slot until the kernel ends (kwarg update_persistent=1 restores it, for A/B) */                    \
-    const int grid = grid_warps((n + 31) / 32, 8, (shard || !g_update_persistent) ? (1 << 22) : num_sms() * 8);  \
     if (shard)       { if (valued) DFB_BU_(K, true, 2, false); else DFB_BU_(K, false, 2, false); }         \
     else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true); else DFB_BU_(K, false, 0, true); }           \
     else             { if (valued) DFB_BU_(K, true, 0, false); else DFB_BU_(K, false, 0, false); }         \

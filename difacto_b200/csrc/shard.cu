@@ -426,7 +426,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   if (max_rows == 0 || max_nnz == 0 || max_nnz > 0x7fffffffULL || max_rows > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "max_rows / max_nnz out of range");
   const int K = h->prm.V_dim;
-  if (!(fm_fast_supported(K) && h->scatter_sorted && !h->force_generic && h->tab.ks == K))
+  if (!h->sorted_path())
     return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in {8,16,32,64,128} and scatter=sorted "
                                     "(other configurations: the all_to_all ShardedStore)");
   DFB_CUDA(h, cudaSetDevice(h->device));

@@ -10,7 +10,7 @@ All ranks share one GPU (engines of one process, phases interleaved as in shard_
   * the benchmark's own batches (bench.gen_raw_batch) and hyper-parameters (bench.hyper): criteo39 with full-size
     segments (criteo_conf, allV, ftrl_l1) and the synthetic workload with id_bits = 30;
   * reversed keys at the ownership boundaries w*s - 1, w*s, w*s + 1 (w = ~0 / S) and the largest key, S = 2, 3, 4;
-  * bit-for-bit invariance: a second run, l2_hints 0 / 1, update_persistent 1 / 0;
+  * bit-for-bit invariance: a second run, l2_hints 0 / 1;
   * S = 1 against the single-GPU raw step at every V_dim.
 Tolerances as in test_gpu_fused_shard.py (shard_sim.STATE_TOL, check_progress: loss 1e-4 relative), with two
 exceptions (LOOSE) that come from column lists hundreds of rows long: the simulation adds their gradients up in
@@ -196,20 +196,14 @@ def assert_same(a, b, what):
     assert a[2] == b[2] and a[3] == b[3], f"{what}: rng state / table"
 
 
-def test_bit_identical_across_runs_l2_hints_and_persistent_update():
+def test_bit_identical_across_runs_and_l2_hints():
     kw = dict(KW, V_dim=64)
     fn = mixed_fn()
     S, steps = 2, 3
     keys = all_keys(S, steps, fn)
-    # update_persistent is process-wide and set by dfb_create: its ranks run alone, and every engine created after them
-    # passes update_persistent=0 explicitly
-    engines, prog = run_local(S, kw, steps, fn, engine_kw=dict(update_persistent=1, l2_hints=1), **MIXED_CAP)
-    persistent = outcome(engines, prog, keys)
-    for E in engines:
-        E.close()
     runs = {}
     for name, ekw in (("hints", dict(l2_hints=1)), ("again", dict(l2_hints=1)), ("no hints", dict(l2_hints=0))):
-        engines, prog = run_local(S, kw, steps, fn, engine_kw=dict(update_persistent=0, **ekw), **MIXED_CAP)
+        engines, prog = run_local(S, kw, steps, fn, engine_kw=ekw, **MIXED_CAP)
         runs[name] = outcome(engines, prog, keys)
         if name == "hints":
             check_vs_simulation(engines, prog, kw, steps, fn, name, **LOOSE)
@@ -217,7 +211,6 @@ def test_bit_identical_across_runs_l2_hints_and_persistent_update():
             E.close()
     assert_same(runs["hints"], runs["again"], "second run")
     assert_same(runs["hints"], runs["no hints"], "l2_hints=0")
-    assert_same(runs["hints"], persistent, "update_persistent=1")
 
 
 @pytest.mark.parametrize("K", [8, 16, 32, 64, 128])

@@ -1,8 +1,8 @@
 """The L2 plan of the single-GPU training step (engine kwarg l2_hints): when the table rows a step touches exceed the L2,
 the fused update keeps p*XV / p evict_last, streams the [V|cg] rows evict_first (k_bwd_update<K, VAL, true, 0, true>,
 k_hot_reduce under the hint) and then drops p*XV / p from L2 with discard.global.L2 (k_l2_discard).  Cache policies
-must not change a single bit: with the plan on, the model equals the one trained with l2_hints=0 and with the
-grid-stride update (update_persistent=1) bit for bit, and the oracle within the suite's tolerances.
+must not change a single bit: with the plan on, the model equals the one trained with l2_hints=0 bit for bit, and
+the oracle within the suite's tolerances.
 
 The batch shapes are computed from the device's L2 and the rule of step_dev (engine.cu): the plan is on when
 u_bound * rs * 4 bytes > L2, where rs = 2 V_dim floats and u_bound is the batch's nnz for a raw step (capped at
@@ -85,17 +85,13 @@ def test_l2_plan_bit_identical_and_vs_oracle(K, valued, above):
     assert n_plan == (3 if above else 0) + plan_on(int(small[0][-1]), K)
 
     kw = dict(V_dim=K, table_capacity=1 << 20, **KW)
-    # update_persistent (like lookup_ilp / lookup_ctas) is process-wide and set by dfb_create: the grid-stride engine
-    # runs alone, and the engines created after it pass the default explicitly
-    P = capi.Engine(update_persistent=1, **kw)
-    prog_p = run(P, seq)
-    H = capi.Engine(update_persistent=0, l2_hints=1, **kw)
-    N = capi.Engine(update_persistent=0, l2_hints=0, **kw)
+    H = capi.Engine(l2_hints=1, **kw)
+    N = capi.Engine(l2_hints=0, **kw)
     M = O.Oracle(V_dim=K, **KW)
     lc_h, lc_n = H.launch_count(), N.launch_count()
     prog_h, prog_n = run(H, seq), run(N, seq)
     assert (H.launch_count() - lc_h) - (N.launch_count() - lc_n) == n_plan      # one k_l2_discard per planned step
-    assert prog_h == prog_n and prog_h == prog_p
+    assert prog_h == prog_n
     for t, (((o, l, i, v), is_train), ph) in enumerate(zip(seq, prog_h)):
         ref = M.sgd_step(o, i, v, l, is_train, is_train)
         assert ph[3] == ref[4]
@@ -105,9 +101,9 @@ def test_l2_plan_bit_identical_and_vs_oracle(K, valued, above):
         assert abs(ph[1] - ref[1]) <= 3e-2 * abs(ref[1]) + 1e-5, f"penalty step {t}: {ph[1]} vs {ref[1]}"
     keys = np.unique(np.concatenate([O.reverse_bytes_np(b[2]) for b, _ in seq]))
     eh = H.read_entries(keys)
-    for a, b, c in zip(eh, N.read_entries(keys), P.read_entries(keys)):
-        assert np.array_equal(a, b) and np.array_equal(a, c)
-    assert H.rng_state() == N.rng_state() == P.rng_state() == M.seed()
+    for a, b in zip(eh, N.read_entries(keys)):
+        assert np.array_equal(a, b)
+    assert H.rng_state() == N.rng_state() == M.seed()
     scal, hasv, V, cg = eh
     oscal, ohasv, oV, ocg = oracle_state(M, keys)
     assert np.array_equal(hasv, ohasv) and (hasv == 1).sum() > len(keys) // 4

@@ -561,26 +561,3 @@ def test_full_size_training_steps_vs_oracle():
     sample = np.unique(np.concatenate([rng.choice(allk, 4000, replace=False), allk[np.argsort(cnt)[-200:]]]))
     hasv = compare_state(M, E, sample)
     assert (hasv > 0).sum() > 200 and (hasv <= 0).sum() > 200      # both kinds of keys were compared
-
-
-def test_k1_bulk_copy_variant_equals_register_staged_kernel():
-    """the cp.async.bulk / mbarrier staged gather kernel (kernels_fm_tma.cu, engine kwarg k1_tma=1; the A/B of
-    DESIGN.md section 3) predicts exactly what k_fm_fast predicts: ragged rows, empty rows, absent V rows, values"""
-    rng = np.random.default_rng(31)
-    kw = dict(V_dim=64, l1=0.02, l2=0.01, lr=0.1, V_lr=0.05, V_threshold=2, V_l2=0.01, V_init_scale=0.1, seed=5)
-    train = [rand_batch(rng, 400, 70, 900, j % 2 == 0) for j in range(3)]
-    val = [rand_batch(rng, 300, 90, 900, j % 2 == 1) for j in range(2)]
-    outs = []
-    for tma in (0, 1):
-        E = engine(k1_tma=tma, **kw)
-        for ep in range(2):
-            for (o, l, i, v) in train:
-                E.train_step_raw(o, i, v, l, push_cnt=(ep == 0), is_train=True)
-        res = []
-        for (o, l, i, v) in val:
-            pr, pred = E.train_step_raw(o, i, v, l, push_cnt=False, is_train=False, want_pred=True)
-            res.append((pr.loss, pred.copy()))
-        outs.append(res)
-    for (l0, p0), (l1, p1) in zip(*outs):
-        assert_close(p1, p0, what="pred (bulk-copy vs LDG)", rtol=1e-6, atol=1e-6)
-        assert abs(l0 - l1) <= 1e-5 * abs(l0)
