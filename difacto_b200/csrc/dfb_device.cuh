@@ -112,6 +112,16 @@ __device__ __forceinline__ void adagrad_step(const Params& p, float gV, float& v
   v = __fsub_rn(v, __fmul_rn(eta, g));
 }
 
+// AdaGrad on one float4 of a V row, grad = g - vp * xp (fm_loss.h:181-198).  PAD: only the first nact (>= 1) columns
+// are V_dim's; the pad columns after them stay as they are (0) -- with V_lr_beta = 0 the step would divide by cg = 0
+template <bool PAD>
+__device__ __forceinline__ void adagrad4(const Params& p, float4 g, float4 vp, float xp, float4& v, float4& c, int nact) {
+  adagrad_step(p, __fsub_rn(g.x, __fmul_rn(vp.x, xp)), v.x, c.x);
+  if (!PAD || nact > 1) adagrad_step(p, __fsub_rn(g.y, __fmul_rn(vp.y, xp)), v.y, c.y);
+  if (!PAD || nact > 2) adagrad_step(p, __fsub_rn(g.z, __fmul_rn(vp.z, xp)), v.z, c.z);
+  if (!PAD || nact > 3) adagrad_step(p, __fsub_rn(g.w, __fmul_rn(vp.w, xp)), v.w, c.w);
+}
+
 // penalty of one w (sgd_learner.cc:257 ; evaluated in fp32 here, double there)
 __device__ __forceinline__ float pen_w(const Params& p, float w) {
   return p.l1 * fabsf(w) + 0.5f * p.l2 * w * w;

@@ -13,6 +13,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 namespace dfb {
 
 struct __align__(32) Entry {
@@ -104,7 +106,7 @@ struct SegDst {
 struct ShardApply {
   const float* w_pulled;        // w of every key as pulled at step start (penalty of the pulled weights)
   const unsigned char* conf;    // != 0: a lower-rank worker's push already updated this key in this step ...
-  const float* vsave;           // ... and this is its V row as pulled at step start ([n][K])
+  const float* vsave;           // ... and this is its V row as pulled at step start ([n][ks])
 };
 
 // very hot keys (a Criteo feature that occurs in most rows of a batch): their occurrence lists are cut into chunks
@@ -112,7 +114,7 @@ struct ShardApply {
 // 65536-row list; k_bwd_update then adds the chunk partials in chunk order (bit-reproducible)
 struct HotPart {
   const int* hotmap;        // per key: first chunk id (only valid for keys longer than `split`), < 0: not pre-reduced
-  const float* part;        // [chunks][K] partial sum_occ x * pXV[row]
+  const float* part;        // [chunks][ks] partial sum_occ x * pXV[row]
   const float2* part_s;     // [chunks] partial {sum x p, sum x^2 p}
   int split, chunk;         // lists longer than split are cut into chunks of `chunk` occurrences; part == nullptr: off
 };
@@ -142,7 +144,7 @@ struct PartSrc {
   const float* rval;        // values (nullptr: binary)
   const int2* wv;           // pulled view {bits(w), vrow} of the segment's keys
   const ShardHdr* hdr;      // nrows of the worker's batch
-  float* out_xv;            // [nrows][K]   (peer memory)
+  float* out_xv;            // [nrows][ks]   (peer memory)
   float2* out_sc;           // [nrows] {sum (xV)^2, sum x w}
 };
 struct PartArgs {
@@ -166,7 +168,7 @@ struct FmBatch {
   // emit mode (train && emit): instead of scattering with atomics the kernel writes
   int emit;
   float* p_out;             //   p_i = -y/(1+exp(y pred_i))            [nrows]
-  float* pxv_out;           //   p_i * XV_i                             [nrows][V_dim]
+  float* pxv_out;           //   p_i * XV_i                             [nrows][ks]
   uint32_t* occ_row;        //   row of every nnz (binary data)         [nnz]
   unsigned long long* occ_rowx;  // (row << 32 | bits(x)) (valued data) [nnz]
   // long rows (predict / emit on the fast path): rows of >= long_nnz nonzeros are left to k_fm_long, where a whole
@@ -179,8 +181,32 @@ struct FmBatch {
   const unsigned long long* dev_nkeys;
 };
 
-// true when launch_fm would take the 16-byte-lane fast path for this V_dim / view
+// true when the specialised (16-byte-lane) kernels serve this V_dim: 0 <= V_dim <= 128
 bool fm_fast_supported(int V_dim);
+
+// The specialised kernels' lane-group width for a V_dim: the smallest K in {8,16,32,64,128} with K >= V_dim (V_dim 0:
+// 8), 0 above 128.  A row is handled by K/4 lanes of one float4 each; every per-row buffer has the stride
+// ks = V_dim rounded up to 4 <= K, and the lanes whose float4 starts at or beyond ks load and store nothing.  The
+// kernels take that predicate as a template flag PAD = (V_dim != K): their PAD = false instantiations are the
+// exact-width code.
+inline int fast_lane_width(int V_dim) {
+  if (V_dim < 0 || V_dim > 128) return 0;
+  int K = 8;
+  while (K < V_dim) K *= 2;
+  return K;
+}
+// f(std::integral_constant<int, K>{}) for K = fast_lane_width(V_dim); -1 when V_dim has no fast kernels
+template <typename F>
+int with_lane_width(int V_dim, F&& f) {
+  switch (fast_lane_width(V_dim)) {
+    case 8: return f(std::integral_constant<int, 8>{});
+    case 16: return f(std::integral_constant<int, 16>{});
+    case 32: return f(std::integral_constant<int, 32>{});
+    case 64: return f(std::integral_constant<int, 64>{});
+    case 128: return f(std::integral_constant<int, 128>{});
+  }
+  return -1;
+}
 
 // streaming multiprocessors of the current device (cached per device); the grid-stride kernels cap their
 // grids at a multiple of it

@@ -200,8 +200,7 @@ namespace {
 
 // the fused minibatch on device-resident inputs (everything enqueued on h->stream)
 int ensure_sorted_ws(dfb_engine* h, size_t nrows, size_t nnz, size_t U, bool valued, bool csc_given = false) {
-  const int k = h->prm.V_dim;
-  DFB_TRY(h->ensure(h->pxv, nrows * (size_t)k * sizeof(float)));
+  DFB_TRY(h->ensure(h->pxv, nrows * (size_t)h->tab.ks * sizeof(float)));
   DFB_TRY(h->ensure(h->p_row, nrows * sizeof(float)));
   if (csc_given) return 0;
   DFB_TRY(h->ensure(h->occ, nnz * (valued ? 8 : 4)));
@@ -350,7 +349,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "sorted scatter unsupported for this V_dim");
     h->launches += nl;
     if (l2_plan)
-      h->launches += launch_l2_discard(h->pxv.p, nrows * (size_t)h->prm.V_dim * sizeof(float), h->p_row.p,
+      h->launches += launch_l2_discard(h->pxv.p, nrows * (size_t)ks * sizeof(float), h->p_row.p,
                                        nrows * sizeof(float), s);
     h->launches += launch_initv(h->tab, h->prm, slot, U, dU, flags, pos, s);
   } else if (is_train) {
@@ -1531,7 +1530,7 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
   for (int i = 0; i < nseg; ++i) { sd.gw[i] = peer_gw[i]; sd.gV[i] = peer_gV[i]; }
   if (first_seg >= 0 && first_seg < nseg) sd.rot = sd.bounds[first_seg] / 32 * 32;
   if ((size_t)sd.bounds[nseg] != nkeys) return h->fail(DFB_ERR_INVALID, "seg_bounds[nseg] must equal nkeys");
-  if (!h->sorted_path())
+  if (!h->sorted_path() || fast_lane_width(h->prm.V_dim) != h->prm.V_dim)
     return h->fail(DFB_ERR_INVALID, "peer gradient stores need the sorted scatter path (V_dim in {8,16,32,64,128})");
   return dev_fm_step_impl(h, nrows, nnz, d_offset, d_index, d_value, d_label, nkeys, d_w, d_hasv, d_V, 1,
                           peer_gw[0], peer_gV[0], &sd);
@@ -1547,7 +1546,8 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
   const int ks = h->tab.ks, k = h->prm.V_dim;
   if (nkeys > 0x7fffffffULL || nrows > 0x7fffffffULL || nnz > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "batch too large");
-  const bool sorted = is_train && h->sorted_path();
+  // the worker's dense gradient rows (launch_bwd_dense) exist at the exact widths only
+  const bool sorted = is_train && h->sorted_path() && fast_lane_width(k) == k;
   DFB_TRY(h->ensure(h->pred, nrows * sizeof(float)));
   FmView v;
   memset(&v, 0, sizeof(v));

@@ -94,7 +94,7 @@ struct dfb_engine {
   unsigned long long* h_nvals = nullptr;  // pinned
   ShardState* shard = nullptr;          // the NVLink-sharded store this engine is a rank of (shard.cu)
 
-  // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (V_dim in {8,16,32,64,128}) and,
+  // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (0 <= V_dim <= 128) and,
   // when it trains, the atomic-free sorted gradient reduction
   bool sorted_path(bool is_train = true) const {
     return !force_generic && dfb::fm_fast_supported(prm.V_dim) && (!is_train || scatter_sorted);

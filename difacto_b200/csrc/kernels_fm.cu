@@ -86,6 +86,8 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 // ---------------------------------------------------------------------------------------
 // fast path: K in {8,16,32,64,128}, 16-byte aligned rows
 // ---------------------------------------------------------------------------------------
+// PAD (V_dim < K, see fast_lane_width): the rows have stride ks = V_dim rounded up to 4, lanes whose float4 starts at
+// or beyond ks load and store nothing, and V_dim 0 leaves the prediction unclamped (fm_loss.h:77)
 // MODE 0: predict only.  MODE 1: training with fp32 red.global scatter into dense gradient rows.
 // MODE 2: training, "emit": writes p_i, p_i*XV_i and the (row[,x]) payload of every nnz so that
 //         the gradient can be reduced per key without atomics (kernels_table.cu: k_bwd_update).
@@ -100,9 +102,10 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 #ifndef DFB_FM_MINBLOCKS32
 #define DFB_FM_MINBLOCKS32 DFB_FM_MINBLOCKS     // V_dim = 32 (tuning builds: 3 removes its ~130-byte spills)
 #endif
-template <int K, int MODE, bool HAS_VAL>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false>
 __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MINBLOCKS) k_fm_fast(FmBatch b, FmView v, PartArgs pa) {
   constexpr bool TRAIN = MODE == 1;
+  static_assert(!(PAD && TRAIN), "the atomic scatter runs the exact widths only");
   constexpr int LPR = K / 4;                 // lanes per V row, one float4 each
   constexpr int G = 32 / LPR;                // V rows fetched by one warp-wide load
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;   // independent loads in flight per lane
@@ -110,6 +113,8 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
   if (MODE != 3 && batch_dropped(b, true)) return;
   const int lane = threadIdx.x & 31;
   const int sub = lane % LPR, grp = lane / LPR;
+  const int ks = PAD ? (b.V_dim + 3) / 4 * 4 : K;
+  const bool act = !PAD || sub * 4 < ks;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
   float loss_acc = 0.f;
@@ -183,7 +188,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
           const int t = t0 + q * G + grp;
           const int vr_t = __shfl_sync(kFull, vr, t & 31);
           const float x_t = __shfl_sync(kFull, x, t & 31);
-          const bool ok = (t < cnt) && (vr_t >= 0);
+          const bool ok = (t < cnt) && (vr_t >= 0) && act;
           xs[q] = ok ? x_t : 0.f;
           vv[q] = ok ? ldg128_pol(v.vbase + (long long)vr_t * v.vstride + sub * 4, pol_v)
                      : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -210,7 +215,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
     wsum = warp_sum(wsum);
     if (MODE == 3) {
       // ||XV||^2 is not linear in the rows: the worker squares the SUM of the owners' partials
-      if (grp == 0) *reinterpret_cast<float4*>(pa.s[src].out_xv + row * (size_t)K + sub * 4) = xv;
+      if (grp == 0 && act) *reinterpret_cast<float4*>(pa.s[src].out_xv + row * (size_t)ks + sub * 4) = xv;
       if (lane == 0) pa.s[src].out_sc[row] = make_float2(acc2, wsum);
       continue;
     }
@@ -218,7 +223,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
     s1 = warp_sum(s1);
     float pred = (b.pred_acc ? b.pred_io[row] : 0.f) + wsum;
     pred += 0.5f * (s1 - acc2);
-    pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:118
+    if (!PAD || b.V_dim > 0) pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:77,118
     const float label = b.label ? __ldg(b.label + row) : 0.f;
     if (lane == 0) {
       if (b.pred_io) b.pred_io[row] = pred;
@@ -227,9 +232,9 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
     if (MODE == 2) {
       const float p = row_p(label, pred);
       if (lane == 0) b.p_out[row] = p;
-      // XV_ *= p (fm_loss.h:191-195), one coalesced 4K-byte row
-      if (grp == 0)
-        *reinterpret_cast<float4*>(b.pxv_out + row * (size_t)K + sub * 4) =
+      // XV_ *= p (fm_loss.h:191-195), one coalesced 4ks-byte row
+      if (grp == 0 && act)
+        *reinterpret_cast<float4*>(b.pxv_out + row * (size_t)ks + sub * 4) =
             make_float4(p * xv.x, p * xv.y, p * xv.z, p * xv.w);
     }
 
@@ -276,7 +281,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
 // ---------------------------------------------------------------------------------------
 constexpr int kLongWarps = 8;
 
-template <int K, int MODE, bool HAS_VAL>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false>
 __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v, int scan_rows) {
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
@@ -286,6 +291,8 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
   if (batch_dropped(b, false)) return;                // k_fm_fast reports it
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int sub = lane % LPR, grp = lane / LPR;
+  const int ks = PAD ? (b.V_dim + 3) / 4 * 4 : K;
+  const bool act = !PAD || sub * 4 < ks;
   const uint64_t pol_v = l2_policy(v.l2hint ? kL2EvictFirst : kL2Normal);
   const uint64_t pol_wv = l2_policy(v.wv_last ? kL2EvictLast : kL2Normal);
   float loss_acc = 0.f;                       // thread 0 only
@@ -338,7 +345,7 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
             const int t = t0 + q * G + grp;
             const int vr_t = __shfl_sync(kFull, vr, t & 31);
             const float x_t = __shfl_sync(kFull, x, t & 31);
-            const bool ok = (t < cnt) && (vr_t >= 0);
+            const bool ok = (t < cnt) && (vr_t >= 0) && act;
             xs[q] = ok ? x_t : 0.f;
             vv[q] = ok ? ldg128_pol(v.vbase + (long long)vr_t * v.vstride + sub * 4, pol_v)
                        : make_float4(0.f, 0.f, 0.f, 0.f);
@@ -378,7 +385,7 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
         s1 = warp_sum(s1);
         float pred = (b.pred_acc ? b.pred_io[row] : 0.f) + ws;
         pred += 0.5f * (s1 - a2);
-        pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:118
+        if (!PAD || b.V_dim > 0) pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:77,118
         const float label = b.label ? __ldg(b.label + row) : 0.f;
         if (lane == 0) {
           if (b.pred_io) b.pred_io[row] = pred;
@@ -387,8 +394,8 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
         if (MODE == 2) {
           const float p = row_p(label, pred);
           if (lane == 0) b.p_out[row] = p;
-          if (grp == 0)
-            *reinterpret_cast<float4*>(b.pxv_out + row * (size_t)K + sub * 4) = make_float4(p * t.x, p * t.y, p * t.z, p * t.w);
+          if (grp == 0 && act)
+            *reinterpret_cast<float4*>(b.pxv_out + row * (size_t)ks + sub * 4) = make_float4(p * t.x, p * t.y, p * t.z, p * t.w);
         }
       }
       __syncthreads();
@@ -531,7 +538,7 @@ __global__ void k_grad_finalize_dense(int k, int ks, size_t nkeys, const int* ha
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-template <int K>
+template <int K, bool PAD>
 int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const int threads = 256;
   size_t need = (b.nrows + 7) / 8;
@@ -540,14 +547,15 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   PartArgs pa;
   memset(&pa, 0, sizeof(pa));
   if (b.train && b.emit) {
-    if (hv) k_fm_fast<K, 2, true><<<grid, threads, 0, s>>>(b, v, pa);
-    else    k_fm_fast<K, 2, false><<<grid, threads, 0, s>>>(b, v, pa);
+    if (hv) k_fm_fast<K, 2, true, PAD><<<grid, threads, 0, s>>>(b, v, pa);
+    else    k_fm_fast<K, 2, false, PAD><<<grid, threads, 0, s>>>(b, v, pa);
   } else if (b.train) {
-    if (hv) k_fm_fast<K, 1, true><<<grid, threads, 0, s>>>(b, v, pa);
-    else    k_fm_fast<K, 1, false><<<grid, threads, 0, s>>>(b, v, pa);
+    if constexpr (PAD) return -1;      // (launch_fm sends the atomic scatter to the generic kernel)
+    else if (hv) k_fm_fast<K, 1, true><<<grid, threads, 0, s>>>(b, v, pa);
+    else         k_fm_fast<K, 1, false><<<grid, threads, 0, s>>>(b, v, pa);
   } else {
-    if (hv) k_fm_fast<K, 0, true><<<grid, threads, 0, s>>>(b, v, pa);
-    else    k_fm_fast<K, 0, false><<<grid, threads, 0, s>>>(b, v, pa);
+    if (hv) k_fm_fast<K, 0, true, PAD><<<grid, threads, 0, s>>>(b, v, pa);
+    else    k_fm_fast<K, 0, false, PAD><<<grid, threads, 0, s>>>(b, v, pa);
   }
   // rows of >= long_nnz nonzeros: one CTA each (the scan over the offsets costs ~1 us when there is none)
   if (b.long_nnz && (!b.train || b.emit) && (b.nnz_hint == 0 || b.nnz_hint >= b.long_nnz)) {
@@ -555,59 +563,59 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
     int scan = 1;
     while (scan < kLongWarps * 32 && (size_t)lgrid * scan * 2 <= b.nrows) scan *= 2;
     if (b.train) {
-      if (hv) k_fm_long<K, 2, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
-      else    k_fm_long<K, 2, false><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      if (hv) k_fm_long<K, 2, true, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      else    k_fm_long<K, 2, false, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
     } else {
-      if (hv) k_fm_long<K, 0, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
-      else    k_fm_long<K, 0, false><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      if (hv) k_fm_long<K, 0, true, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      else    k_fm_long<K, 0, false, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
     }
     return 2;
   }
   return 1;
 }
 
-template <int K>
-int launch_partial_k(bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s) {
+template <int K, bool PAD>
+int launch_partial_k(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s) {
   FmBatch b;
   memset(&b, 0, sizeof(b));
-  b.V_dim = K;
+  b.V_dim = V_dim;
   const int grid = num_sms() * 8;
-  if (valued) k_fm_fast<K, 3, true><<<grid, 256, 0, s>>>(b, v, pa);
-  else        k_fm_fast<K, 3, false><<<grid, 256, 0, s>>>(b, v, pa);
+  if constexpr (PAD) {
+    if (!valued) return -1;       // the owners' wire format is always valued (kernels_shard.cu)
+    k_fm_fast<K, 3, true, true><<<grid, 256, 0, s>>>(b, v, pa);
+  } else {
+    if (valued) k_fm_fast<K, 3, true><<<grid, 256, 0, s>>>(b, v, pa);
+    else        k_fm_fast<K, 3, false><<<grid, 256, 0, s>>>(b, v, pa);
+  }
   return 1;
 }
 
 }  // namespace
 
-bool fm_fast_supported(int k) { return k == 8 || k == 16 || k == 32 || k == 64 || k == 128; }
+bool fm_fast_supported(int k) { return fast_lane_width(k) != 0; }
 
 int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s) {
-  switch (V_dim) {
-    case 8: return launch_partial_k<8>(valued, v, pa, s);
-    case 16: return launch_partial_k<16>(valued, v, pa, s);
-    case 32: return launch_partial_k<32>(valued, v, pa, s);
-    case 64: return launch_partial_k<64>(valued, v, pa, s);
-    case 128: return launch_partial_k<128>(valued, v, pa, s);
-  }
-  return -1;
+  return with_lane_width(V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    return V_dim == K ? launch_partial_k<K, false>(V_dim, valued, v, pa, s)
+                      : launch_partial_k<K, true>(V_dim, valued, v, pa, s);
+  });
 }
 
 int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s) {
   const int k = b.V_dim;
-  bool fast = !force_generic && (k == 8 || k == 16 || k == 32 || k == 64 || k == 128) &&
+  bool fast = !force_generic && fm_fast_supported(k) &&
               v.v_pos != nullptr && aligned16(v.vbase) && (v.vstride % 4 == 0);
-  if (fast && b.train && !b.emit) {
-    fast = aligned16(v.gvbase) && (v.gvstride % 4 == 0) && (b.value == nullptr || v.gxxp != nullptr);
+  if (fast && b.train && !b.emit) {      // the atomic scatter: exact widths only
+    fast = fast_lane_width(k) == k && aligned16(v.gvbase) && (v.gvstride % 4 == 0) &&
+           (b.value == nullptr || v.gxxp != nullptr);
   }
   if (b.train && b.emit && !fast) return -1;   // the emit mode exists only on the fast path
   if (fast) {
-    switch (k) {
-      case 8: return launch_fast_k<8>(b, v, s);
-      case 16: return launch_fast_k<16>(b, v, s);
-      case 32: return launch_fast_k<32>(b, v, s);
-      case 64: return launch_fast_k<64>(b, v, s);
-      case 128: return launch_fast_k<128>(b, v, s);
-    }
+    return with_lane_width(k, [&](auto kc) {
+      constexpr int K = decltype(kc)::value;
+      return k == K ? launch_fast_k<K, false>(b, v, s) : launch_fast_k<K, true>(b, v, s);
+    });
   }
   if (k > 0 && v.v_pos == nullptr) return -1;   // V_pos is required when V_dim > 0
   const int threads = 128;

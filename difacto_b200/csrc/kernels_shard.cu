@@ -270,8 +270,9 @@ __global__ void __launch_bounds__(256) k_shard_fill(const uint64_t* __restrict__
 }
 
 // add the owners' partials, finish Predict / Evaluate / p (fm_loss.h:108-118,155-161; loss.h:57-66) and send
-// p_i and p_i * XV_i to every owner.  LPR lanes (one float4 each) per row, G rows per warp.
-template <int K>
+// p_i and p_i * XV_i to every owner.  LPR lanes (one float4 each) per row, G rows per warp.  PAD: rows of stride
+// ks < K, the lanes beyond it idle, no clamp at V_dim 0 (fm_loss.h:77)
+template <int K, bool PAD = false>
 __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
@@ -280,6 +281,8 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
   // or added to Progress
   if (!a.wb->valid) return;
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
+  const int ks = PAD ? (a.V_dim + 3) / 4 * 4 : K;
+  const bool act = !PAD || sub * 4 < ks;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
   const size_t ntiles = (a.nrows + G - 1) / G;
@@ -291,8 +294,10 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
     float acc2 = 0.f, wsum = 0.f;
     if (ok) {
       for (int s = 0; s < a.S; ++s) {      // fixed order: bit-reproducible
-        const float4 t = *reinterpret_cast<const float4*>(a.part_xv[s] + row * (size_t)K + sub * 4);
-        xv.x += t.x; xv.y += t.y; xv.z += t.z; xv.w += t.w;
+        if (act) {
+          const float4 t = *reinterpret_cast<const float4*>(a.part_xv[s] + row * (size_t)ks + sub * 4);
+          xv.x += t.x; xv.y += t.y; xv.z += t.z; xv.w += t.w;
+        }
         if (sub == 0) { const float2 sc = a.part_sc[s][row]; acc2 += sc.x; wsum += sc.y; }
       }
     }
@@ -302,7 +307,7 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
     acc2 = __shfl_sync(kFullMask, acc2, grp * LPR);
     wsum = __shfl_sync(kFullMask, wsum, grp * LPR);
     float pred = wsum + 0.5f * (s1 - acc2);
-    pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:118
+    if (!PAD || a.V_dim > 0) pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:77,118
     if (!ok) continue;
     const float label = __ldg(a.label + row);
     const float y = label > 0.f ? 1.f : -1.f;
@@ -316,7 +321,7 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
       for (int q = 0; q < a.S; ++q) {
         int s = q + a.me;
         if (s >= a.S) s -= a.S;
-        *reinterpret_cast<float4*>(a.pxv_dst[s] + row * (size_t)K + sub * 4) = g;
+        if (act) *reinterpret_cast<float4*>(a.pxv_dst[s] + row * (size_t)ks + sub * 4) = g;
         if (sub == 0) a.p_dst[s][row] = p;
       }
     }
@@ -400,7 +405,7 @@ __global__ void __launch_bounds__(256) k_shard_lookup(Table t, LookupArgs a, int
 // deletes keeps slots stable).  For a key a lower-rank worker of this step holds too (conf), the pull-time V row is
 // saved: that worker's push will have changed the table row by the time this worker's gradient needs it.
 __global__ void __launch_bounds__(256) k_shard_pull(Table t, LookupArgs a, const unsigned char* __restrict__ conf,
-                                                    float* __restrict__ vsave, int K) {
+                                                    float* __restrict__ vsave, int ks) {
   const int lane = threadIdx.x & 31;
   const size_t warp0 = ((size_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const size_t nwarps = ((size_t)gridDim.x * blockDim.x) >> 5;
@@ -431,8 +436,8 @@ __global__ void __launch_bounds__(256) k_shard_pull(Table t, LookupArgs a, const
       m &= m - 1;
       const int vrb = __shfl_sync(kFullMask, vr_save, b);
       const float4* src = reinterpret_cast<const float4*>(t.V + (size_t)vrb * t.rs);
-      float4* dst = reinterpret_cast<float4*>(vsave + (base + b) * (size_t)K);
-      for (int l = lane; l < K / 4; l += 32) dst[l] = src[l];
+      float4* dst = reinterpret_cast<float4*>(vsave + (base + b) * (size_t)ks);
+      for (int l = lane; l < ks / 4; l += 32) dst[l] = src[l];
     }
   }
 }
@@ -516,22 +521,15 @@ int launch_shard_subcsr(const uint64_t* offset, const uint32_t* lidx, const floa
   return 3;
 }
 
-int launch_shard_reduce(int V_dim, const ReduceArgs& a, cudaStream_t s) {
+int launch_shard_reduce(const ReduceArgs& a, cudaStream_t s) {
   if (a.nrows == 0) return 0;
-#define DFB_RED(K)                                                                             \
-  do {                                                                                         \
-    const size_t tiles = (a.nrows + (32 / (K / 4)) - 1) / (32 / (K / 4));                      \
-    k_shard_reduce<K><<<grid_cap(tiles, 8, num_sms() * 8), 256, 0, s>>>(a);                          \
-  } while (0)
-  switch (V_dim) {
-    case 8: DFB_RED(8); return 1;
-    case 16: DFB_RED(16); return 1;
-    case 32: DFB_RED(32); return 1;
-    case 64: DFB_RED(64); return 1;
-    case 128: DFB_RED(128); return 1;
-  }
-#undef DFB_RED
-  return -1;
+  return with_lane_width(a.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    const size_t tiles = (a.nrows + (32 / (K / 4)) - 1) / (32 / (K / 4));
+    if (a.V_dim == K) k_shard_reduce<K><<<grid_cap(tiles, 8, num_sms() * 8), 256, 0, s>>>(a);
+    else              k_shard_reduce<K, true><<<grid_cap(tiles, 8, num_sms() * 8), 256, 0, s>>>(a);
+    return 1;
+  });
 }
 
 int launch_shard_lookup(Table& t, const LookupArgs& a, int r, bool insert, unsigned char* conf, cudaStream_t s) {
@@ -541,9 +539,9 @@ int launch_shard_lookup(Table& t, const LookupArgs& a, int r, bool insert, unsig
   return 1;
 }
 
-int launch_shard_pull(Table& t, const LookupArgs& a, const unsigned char* conf, float* vsave, int K, cudaStream_t s) {
+int launch_shard_pull(Table& t, const LookupArgs& a, const unsigned char* conf, float* vsave, cudaStream_t s) {
   const size_t total = (size_t)a.S * a.Kseg;
-  k_shard_pull<<<grid_cap((total + 31) / 32, 8, num_sms() * 16), 256, 0, s>>>(t, a, conf, vsave, K);
+  k_shard_pull<<<grid_cap((total + 31) / 32, 8, num_sms() * 16), 256, 0, s>>>(t, a, conf, vsave, t.ks);
   return 1;
 }
 

@@ -663,6 +663,8 @@ __device__ __forceinline__ void load_occ(const void* occ, int o, uint32_t& row, 
 // UNRB row-groups in flight; the first occurrence's p*XV row is fetched together with V|cg.
 // SRC 0: gradient reduced from the occurrence lists (fused step / worker).  SRC 1: gradient read
 // from dense rows gw_in[n], gV_in[n][K] that a worker pushed (owner side of the sharded store).
+// PAD (V_dim < K, single-GPU step and SRC 2 only): lanes at or beyond ks = t.ks touch nothing, the per-row buffers
+// (p*XV, hot-key partials, vsave) have stride ks, and the pad columns [V_dim, ks) of the last float4 are not updated.
 // 3 CTAs/SM (80 registers): at 4 (64 registers) sm_90 spills ~100 bytes per thread and the update stage of the
 // V_dim = 64 training step takes 3.54 ms instead of 3.34 ms (H100 SXM, 700 W)
 #ifndef DFB_BU_MINBLOCKS
@@ -671,7 +673,7 @@ __device__ __forceinline__ void load_occ(const void* occ, int o, uint32_t& row, 
 #ifndef DFB_BU_UNRB
 #define DFB_BU_UNRB 2
 #endif
-template <int K, bool HAS_VAL, bool APPLY, int SRC = 0, bool HINT = false>
+template <int K, bool HAS_VAL, bool APPLY, int SRC = 0, bool HINT = false, bool PAD = false>
 __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, Params p, const int* __restrict__ slot,
                                                     const int* __restrict__ pull_vrow, size_t n_cap,
                                                     const unsigned long long* __restrict__ dn,
@@ -690,7 +692,11 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
   constexpr int NPASS = 32 / G;
   constexpr int UNRB = NPASS >= DFB_BU_UNRB ? DFB_BU_UNRB : 1;
   constexpr int kHeavy = 64;     // occurrence-list length above which a key is reduced cooperatively
+  static_assert(!PAD || (APPLY && SRC != 1), "padded rows: the table-applying update of the fused paths only");
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
+  const int ks = PAD ? t.ks : K;                  // stride of the per-row buffers
+  const bool act = !PAD || sub * 4 < ks;          // this lane's float4 holds V columns
+  const int nact = PAD ? min(4, p.V_dim - sub * 4) : 4;
   const unsigned warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
   // L2 plan of the single-GPU step (dfb_device.cuh): this batch's p*XV rows and p (16.8 MB at the flagship shape) are
@@ -838,7 +844,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
         const float xx0 = __shfl_sync(kFull, x0, kk);
         v[q] = c[q] = g[q] = make_float4(0.f, 0.f, 0.f, 0.f);
         if (o1k[q] - o0k[q] > kHeavy) vrk[q] = -1;      // handled by the whole warp after the passes
-        if (vrk[q] >= 0) {
+        if (vrk[q] >= 0 && act) {
           if (APPLY) {
             const float* Vr = t.V + (size_t)vrk[q] * t.rs + sub * 4;
             v[q] = ld_row(Vr);
@@ -852,7 +858,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
             const size_t ik = base + (unsigned)((pass + q) * G + grp);
             g[q] = __ldg(reinterpret_cast<const float4*>(pxv + ik * (size_t)K + sub * 4));   // pxv aliases gV_in
           } else if (o1k[q] > o0k[q]) {
-            const float4 tt = ld_pxv(pxv + (size_t)r0 * K + sub * 4);
+            const float4 tt = ld_pxv(pxv + (size_t)r0 * ks + sub * 4);
             g[q] = make_float4(__fmul_rn(tt.x, xx0), __fmul_rn(tt.y, xx0), __fmul_rn(tt.z, xx0),
                                __fmul_rn(tt.w, xx0));                                   // spmm.h:152-154
           }
@@ -860,7 +866,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
       }
 #pragma unroll
       for (int q = 0; q < UNRB; ++q) {
-        if (vrk[q] < 0) continue;
+        if (vrk[q] < 0 || !act) continue;
         for (int o = o0k[q] + 1; o < o1k[q]; o += 4) {   // further occurrences: loads 4 ahead, sums in row order
           float4 tt[4]; float xs[4];
 #pragma unroll
@@ -869,7 +875,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
             if (o + r < o1k[q]) {
               uint32_t row;
               load_occ<HAS_VAL, HINT>(occ, o + r, row, xs[r], pol_once);
-              tt[r] = ld_pxv(pxv + (size_t)row * K + sub * 4);
+              tt[r] = ld_pxv(pxv + (size_t)row * ks + sub * 4);
             }
           }
 #pragma unroll
@@ -885,13 +891,9 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
           // only for a key a lower-rank worker's push has already updated in this step (SRC 2)
           float4 vp = v[q];
           if (SRC == 2 && cfk[q])
-            vp = __ldg(reinterpret_cast<const float4*>(sa.vsave + (size_t)(base + (unsigned)((pass + q) * G + grp)) * (size_t)K + sub * 4));
+            vp = __ldg(reinterpret_cast<const float4*>(sa.vsave + (size_t)(base + (unsigned)((pass + q) * G + grp)) * (size_t)ks + sub * 4));
           if (acc_pen) pen += 0.5f * p.V_l2 * (vp.x * vp.x + vp.y * vp.y + vp.z * vp.z + vp.w * vp.w);
-          const float xp = xxpk[q];
-          adagrad_step(p, __fsub_rn(g[q].x, __fmul_rn(vp.x, xp)), v[q].x, c[q].x);
-          adagrad_step(p, __fsub_rn(g[q].y, __fmul_rn(vp.y, xp)), v[q].y, c[q].y);
-          adagrad_step(p, __fsub_rn(g[q].z, __fmul_rn(vp.z, xp)), v[q].z, c[q].z);
-          adagrad_step(p, __fsub_rn(g[q].w, __fmul_rn(vp.w, xp)), v[q].w, c[q].w);
+          adagrad4<PAD>(p, g[q], vp, xxpk[q], v[q], c[q], nact);
           float* Vr = t.V + (size_t)vrk[q] * t.rs + sub * 4;
           st_row(Vr, v[q]);
           st_row(Vr + t.ks, c[q]);
@@ -924,7 +926,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
         const size_t ik = base + (unsigned)hl;
         float4 hv = make_float4(0.f, 0.f, 0.f, 0.f), hc = hv;
         float* Vr = nullptr;
-        if (grp == 0) {
+        if (grp == 0 && act) {
           if (APPLY) {
             Vr = t.V + (size_t)hvr * t.rs + sub * 4;
             hv = ld_row(Vr);
@@ -939,10 +941,10 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
         int first = -1;
         if (hp.part != nullptr && ho1 - ho0 > hp.split) first = hp.hotmap[ik];
         if (first >= 0) {      // pre-reduced in chunks: chunk partials in chunk order
-          if (grp == 0) {
+          if (grp == 0 && act) {
             const int nch = (ho1 - ho0 + hp.chunk - 1) / hp.chunk;
             for (int c = 0; c < nch; ++c) {
-              const float4 tp = __ldg(reinterpret_cast<const float4*>(hp.part + (size_t)(first + c) * K + sub * 4));
+              const float4 tp = __ldg(reinterpret_cast<const float4*>(hp.part + (size_t)(first + c) * ks + sub * 4));
               acc[0].x += tp.x; acc[0].y += tp.y; acc[0].z += tp.z; acc[0].w += tp.w;
             }
           }
@@ -952,10 +954,10 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
 #pragma unroll
           for (int r = 0; r < 4; ++r) {
             xs[r] = 0.f; tt[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (o + r * G < ho1) {
+            if (o + r * G < ho1 && act) {
               uint32_t row;
               load_occ<HAS_VAL, HINT>(occ, o + r * G, row, xs[r], pol_once);
-              tt[r] = ld_pxv(pxv + (size_t)row * K + sub * 4);
+              tt[r] = ld_pxv(pxv + (size_t)row * ks + sub * 4);
             }
           }
 #pragma unroll
@@ -971,16 +973,13 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
           hg.x += __shfl_xor_sync(kFull, hg.x, o); hg.y += __shfl_xor_sync(kFull, hg.y, o);
           hg.z += __shfl_xor_sync(kFull, hg.z, o); hg.w += __shfl_xor_sync(kFull, hg.w, o);
         }
-        if (grp == 0) {
+        if (grp == 0 && act) {
           float4 hp = hv;      // the pulled row (see phase B)
           if (SRC == 2 && hcf)
-            hp = __ldg(reinterpret_cast<const float4*>(sa.vsave + ik * (size_t)K + sub * 4));
+            hp = __ldg(reinterpret_cast<const float4*>(sa.vsave + ik * (size_t)ks + sub * 4));
           if (acc_pen) pen += 0.5f * p.V_l2 * (hp.x * hp.x + hp.y * hp.y + hp.z * hp.z + hp.w * hp.w);
           if (APPLY) {
-            adagrad_step(p, __fsub_rn(hg.x, __fmul_rn(hp.x, hxp)), hv.x, hc.x);
-            adagrad_step(p, __fsub_rn(hg.y, __fmul_rn(hp.y, hxp)), hv.y, hc.y);
-            adagrad_step(p, __fsub_rn(hg.z, __fmul_rn(hp.z, hxp)), hv.z, hc.z);
-            adagrad_step(p, __fsub_rn(hg.w, __fmul_rn(hp.w, hxp)), hv.w, hc.w);
+            adagrad4<PAD>(p, hg, hp, hxp, hv, hc, nact);
             st_row(Vr, hv);
             st_row(Vr + t.ks, hc);
           } else {
@@ -1022,12 +1021,15 @@ __global__ void k_hot_find(const int* __restrict__ col_start, const int* __restr
   }
 }
 
-template <int K, bool HAS_VAL>
+// PAD: rows of stride ks < K (see k_bwd_update)
+template <int K, bool HAS_VAL, bool PAD = false>
 __global__ void __launch_bounds__(256) k_hot_reduce(const void* __restrict__ occ, const float* __restrict__ p_row,
-                                                    const float* __restrict__ pxv, HotWs ws, int l2hint) {
+                                                    const float* __restrict__ pxv, HotWs ws, int l2hint, int ks_pad) {
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
+  const int ks = PAD ? ks_pad : K;
+  const bool act = !PAD || sub * 4 < ks;
   const unsigned warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const unsigned nwarps = (gridDim.x * blockDim.x) >> 5;
   // the L2 plan of k_bwd_update: p*XV / p kept for the update that follows, the occurrence lists streamed
@@ -1055,10 +1057,10 @@ __global__ void __launch_bounds__(256) k_hot_reduce(const void* __restrict__ occ
 #pragma unroll
       for (int r = 0; r < 4; ++r) {
         xs[r] = 0.f; tt[r] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (o + r * G < be.y) {
+        if (o + r * G < be.y && act) {
           uint32_t row;
           load_occ<HAS_VAL, true>(occ, o + r * G, row, xs[r], pol_once);
-          tt[r] = ldg128_pol(pxv + (size_t)row * K + sub * 4, pol_keep);
+          tt[r] = ldg128_pol(pxv + (size_t)row * ks + sub * 4, pol_keep);
         }
       }
 #pragma unroll
@@ -1074,7 +1076,7 @@ __global__ void __launch_bounds__(256) k_hot_reduce(const void* __restrict__ occ
       hg.x += __shfl_xor_sync(kFull, hg.x, o); hg.y += __shfl_xor_sync(kFull, hg.y, o);
       hg.z += __shfl_xor_sync(kFull, hg.z, o); hg.w += __shfl_xor_sync(kFull, hg.w, o);
     }
-    if (grp == 0) *reinterpret_cast<float4*>(ws.part + (size_t)c * K + sub * 4) = hg;
+    if (grp == 0 && act) *reinterpret_cast<float4*>(ws.part + (size_t)c * ks + sub * 4) = hg;
     if (lane == 0) ws.part_s[c] = make_float2(a, HAS_VAL ? b2 : a);
   }
 }
@@ -1204,19 +1206,15 @@ int launch_update_dense(Table& t, const Params& p, const int* slot, const int* p
                         size_t n, const float* gw, const float* gxxp, const float* gV, int* flags,
                         int acc_pen, int xxp_mode, cudaStream_t s) {
   if (n == 0) return 0;
-  const int k = p.V_dim;
-#define DFB_UPD(K)                                                                                   \
-  k_update_fast<K><<<grid_warps((n + (32 / (K / 4)) - 1) / (32 / (K / 4)), 8, num_sms() * 8), 256, 0, s>>>( \
-      t, p, slot, pull_vrow, vrow_is_flag, n, gw, gxxp, gV, flags, acc_pen, xxp_mode)
-  switch (k) {
-    case 8: DFB_UPD(8); return 1;
-    case 16: DFB_UPD(16); return 1;
-    case 32: DFB_UPD(32); return 1;
-    case 64: DFB_UPD(64); return 1;
-    case 128: DFB_UPD(128); return 1;
-    default: break;
-  }
-#undef DFB_UPD
+  // the specialised kernel at the exact widths only (the atomic scatter's update)
+  const int nl = with_lane_width(p.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    if (p.V_dim != K) return -1;
+    k_update_fast<K><<<grid_warps((n + (32 / (K / 4)) - 1) / (32 / (K / 4)), 8, num_sms() * 8), 256, 0, s>>>(
+        t, p, slot, pull_vrow, vrow_is_flag, n, gw, gxxp, gV, flags, acc_pen, xxp_mode);
+    return 1;
+  });
+  if (nl > 0) return nl;
   k_update_dense_generic<<<grid_warps(n, 8, num_sms() * 8), 256, 0, s>>>(t, p, slot, pull_vrow, vrow_is_flag, n, gw,
                                                                   gxxp, gV, flags, acc_pen, xxp_mode);
   return 1;
@@ -1309,30 +1307,31 @@ int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pul
   HotPart hp;
   memset(&hp, 0, sizeof(hp));
   if (hot) hp = *hot;
-#define DFB_BU_(K, VAL, SRC, HINT)                                                                             \
-  k_bwd_update<K, VAL, true, SRC, HINT><<<grid, 256, 0, s>>>(t, p, slot, pull_vrow, n, dn, col_start, col_end,       \
+#define DFB_BU_(K, VAL, SRC, HINT, PAD)                                                                        \
+  k_bwd_update<K, VAL, true, SRC, HINT, PAD><<<grid, 256, 0, s>>>(t, p, slot, pull_vrow, n, dn, col_start, col_end,  \
                                                              occ_sorted, p_row, pxv, flags, acc_pen, nullptr, nullptr, \
                                                              nullptr, noseg, sa, hp)
   // one short-lived CTA per 256 keys, so that the higher-priority streams working on the NEXT step (localizer;
   // worker / lookup streams of the sharded store) get SM slots as CTAs retire -- a grid-stride grid holds every
   // slot until the kernel ends
   const int grid = grid_warps((n + 31) / 32, 8, 1 << 22);
-#define DFB_BU(K)                                                                                          \
-  do {                                                                                                     \
-    if (shard)       { if (valued) DFB_BU_(K, true, 2, false); else DFB_BU_(K, false, 2, false); }         \
-    else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true); else DFB_BU_(K, false, 0, true); }           \
-    else             { if (valued) DFB_BU_(K, true, 0, false); else DFB_BU_(K, false, 0, false); }         \
-  } while (0)
-  switch (p.V_dim) {
-    case 8: DFB_BU(8); return 1;
-    case 16: DFB_BU(16); return 1;
-    case 32: DFB_BU(32); return 1;
-    case 64: DFB_BU(64); return 1;
-    case 128: DFB_BU(128); return 1;
-  }
-#undef DFB_BU
+  return with_lane_width(p.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    if (p.V_dim == K) {
+      if (shard)       { if (valued) DFB_BU_(K, true, 2, false, false); else DFB_BU_(K, false, 2, false, false); }
+      else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true, false); else DFB_BU_(K, false, 0, true, false); }
+      else             { if (valued) DFB_BU_(K, true, 0, false, false); else DFB_BU_(K, false, 0, false, false); }
+    } else {
+      if (shard) {
+        if (!valued) return -1;         // the owners' wire format is always valued (kernels_shard.cu)
+        DFB_BU_(K, true, 2, false, true);
+      }
+      else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true, true); else DFB_BU_(K, false, 0, true, true); }
+      else             { if (valued) DFB_BU_(K, true, 0, false, true); else DFB_BU_(K, false, 0, false, true); }
+    }
+    return 1;
+  });
 #undef DFB_BU_
-  return -1;
 }
 
 int launch_l2_discard(void* a, size_t a_bytes, void* b, size_t b_bytes, cudaStream_t s) {
@@ -1351,20 +1350,19 @@ int launch_hot_prereduce(int V_dim, size_t n, const unsigned long long* dn, cons
   cudaMemsetAsync(ws.counter, 0, sizeof(unsigned long long), s);
   k_hot_find<<<grid_for(n, 256, num_sms() * 8), 256, 0, s>>>(col_start, col_end, n, dn, split, chunk, ws);
   const int grid = num_sms() * 4;
-#define DFB_HR(K)                                                                                \
-  do {                                                                                           \
-    if (valued) k_hot_reduce<K, true><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint);  \
-    else        k_hot_reduce<K, false><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint); \
-  } while (0)
-  switch (V_dim) {
-    case 8: DFB_HR(8); break;
-    case 16: DFB_HR(16); break;
-    case 32: DFB_HR(32); break;
-    case 64: DFB_HR(64); break;
-    case 128: DFB_HR(128); break;
-    default: return 0;
-  }
-#undef DFB_HR
+  const int ks = (V_dim + 3) / 4 * 4;
+  const int nl = with_lane_width(V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    if (V_dim == K) {
+      if (valued) k_hot_reduce<K, true><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint, ks);
+      else        k_hot_reduce<K, false><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint, ks);
+    } else {
+      if (valued) k_hot_reduce<K, true, true><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint, ks);
+      else        k_hot_reduce<K, false, true><<<grid, 256, 0, s>>>(occ_sorted, p_row, pxv, ws, l2hint, ks);
+    }
+    return 1;
+  });
+  if (nl < 0) return 0;
   hp->hotmap = ws.hotmap; hp->part = ws.part; hp->part_s = ws.part_s; hp->split = split; hp->chunk = chunk;
   return 2;
 }
@@ -1384,23 +1382,16 @@ int launch_bwd_dense(const Params& p, DevProgress* prog, int ks, const float* w_
   memset(&nosa, 0, sizeof(nosa));
   HotPart nohp;
   memset(&nohp, 0, sizeof(nohp));
-#define DFB_BD(K)                                                                                          \
-  do {                                                                                                     \
-    const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);                                                \
-    if (valued) k_bwd_update<K, true, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end, \
-                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);     \
-    else k_bwd_update<K, false, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end, \
-                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);     \
-  } while (0)
-  switch (p.V_dim) {
-    case 8: DFB_BD(8); return 1;
-    case 16: DFB_BD(16); return 1;
-    case 32: DFB_BD(32); return 1;
-    case 64: DFB_BD(64); return 1;
-    case 128: DFB_BD(128); return 1;
-  }
-#undef DFB_BD
-  return -1;
+  return with_lane_width(p.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    if (p.V_dim != K) return -1;        // exact widths only
+    const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);
+    if (valued) k_bwd_update<K, true, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end,
+                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);
+    else k_bwd_update<K, false, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end,
+                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);
+    return 1;
+  });
 }
 
 // owner side of Push(kGradient) for the specialised V_dims: same phase A/B kernel, gradient read
@@ -1414,21 +1405,14 @@ int launch_update_pushed(Table& t, const Params& p, const int* slot, const int* 
   memset(&nosa, 0, sizeof(nosa));
   HotPart nohp;
   memset(&nohp, 0, sizeof(nohp));
-#define DFB_UP(K)                                                                                          \
-  do {                                                                                                     \
-    const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);                                                \
-    k_bwd_update<K, false, true, 1><<<grid, 256, 0, s>>>(t, p, slot, hasv, n, nullptr, nullptr, nullptr, nullptr, gw, \
-                                                          gV, flags, 0, nullptr, nullptr, nullptr, noseg, nosa, nohp); \
-  } while (0)
-  switch (p.V_dim) {
-    case 8: DFB_UP(8); return 1;
-    case 16: DFB_UP(16); return 1;
-    case 32: DFB_UP(32); return 1;
-    case 64: DFB_UP(64); return 1;
-    case 128: DFB_UP(128); return 1;
-  }
-#undef DFB_UP
-  return -1;
+  return with_lane_width(p.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    if (p.V_dim != K) return -1;        // exact widths only
+    const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);
+    k_bwd_update<K, false, true, 1><<<grid, 256, 0, s>>>(t, p, slot, hasv, n, nullptr, nullptr, nullptr, nullptr, gw,
+                                                          gV, flags, 0, nullptr, nullptr, nullptr, noseg, nosa, nohp);
+    return 1;
+  });
 }
 
 int launch_restore(Table& t, const uint64_t* keys, size_t n, const float* scal, const int* vrow,

@@ -121,7 +121,7 @@ int shard_phase(dfb_engine* h, int phase) {
   cudaEvent_t inputs_ready = c.inputs_ready, consumed = c.consumed;
   LookupArgs& la = c.la;
   const ShardLayout& lay = sh.lay;
-  const int S = sh.S, me = sh.rank, K = h->prm.V_dim;
+  const int S = sh.S, me = sh.rank, K = h->prm.V_dim, ks = h->tab.ks;
   const uint64_t t = sh.step;
   const int d = (int)(t & 1);
   const unsigned long long fv = t + 1;
@@ -225,7 +225,7 @@ int shard_phase(dfb_engine* h, int phase) {
       h->launches += launch_feacnt(h->tab, h->prm, la.slot + (size_t)r * Kseg, Kseg, &hdr[r]->nkeys, nullptr,
                                    lay.at<int>(mine, lay.off_cstart, lay.str_cstart, d, r), flags, ws, O);
   }
-  h->launches += launch_shard_pull(h->tab, la, sh.conf[d].as<unsigned char>(), sh.vsave.as<float>(), K, O);
+  h->launches += launch_shard_pull(h->tab, la, sh.conf[d].as<unsigned char>(), sh.vsave.as<float>(), O);
   DFB_DBG(h, "feacnt / pull view");
   {
     PartArgs pa;
@@ -267,7 +267,7 @@ int shard_phase(dfb_engine* h, int phase) {
     StageTimer tm_red(h, 8, W);
     ReduceArgs ra;
     memset(&ra, 0, sizeof(ra));
-    ra.S = S; ra.me = me; ra.train = is_train ? 1 : 0; ra.nrows = nrows; ra.wb = sh.bounds(d);
+    ra.S = S; ra.me = me; ra.train = is_train ? 1 : 0; ra.V_dim = K; ra.nrows = nrows; ra.wb = sh.bounds(d);
     for (int s = 0; s < S; ++s) {
       ra.part_xv[s] = lay.at<float>(mine, lay.off_part_xv, lay.str_part_xv, d, s);
       ra.part_sc[s] = lay.at<float2>(mine, lay.off_part_sc, lay.str_part_sc, d, s);
@@ -275,7 +275,7 @@ int shard_phase(dfb_engine* h, int phase) {
       ra.pxv_dst[s] = lay.at<float>(sh.peer[s], lay.off_pxv, lay.str_pxv, d, me);
     }
     ra.label = d_lab; ra.pred = sh.pred[d].as<float>(); ra.prog = sh.prog_w(d);
-    int nl = launch_shard_reduce(K, ra, W);
+    int nl = launch_shard_reduce(ra, W);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported V_dim for the sharded store");
     h->launches += nl;
     DFB_DBG(h, "reduce");
@@ -318,7 +318,7 @@ int shard_phase(dfb_engine* h, int phase) {
       ShardApply ap;
       ap.w_pulled = la.w + o;
       ap.conf = la.stamp ? sh.conf[d].as<unsigned char>() + o : nullptr;
-      ap.vsave = sh.vsave.as<float>() + o * (size_t)K;
+      ap.vsave = sh.vsave.as<float>() + o * (size_t)ks;
       const void* occ_r = lay.at<void>(mine, lay.off_occ, lay.str_occ, d, r);
       const float* p_r = lay.at<float>(mine, lay.off_p, lay.str_p, d, r);
       const float* pxv_r = lay.at<float>(mine, lay.off_pxv, lay.str_pxv, d, r);
@@ -425,9 +425,9 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   if (nranks < 1 || nranks > 8 || rank < 0 || rank >= nranks) return h->fail(DFB_ERR_INVALID, "1 <= nranks <= 8, 0 <= rank < nranks");
   if (max_rows == 0 || max_nnz == 0 || max_nnz > 0x7fffffffULL || max_rows > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "max_rows / max_nnz out of range");
-  const int K = h->prm.V_dim;
+  const int ks = h->tab.ks;
   if (!h->sorted_path())
-    return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in {8,16,32,64,128} and scatter=sorted "
+    return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in 0..128, scatter=sorted and no force_generic "
                                     "(other configurations: the all_to_all ShardedStore)");
   DFB_CUDA(h, cudaSetDevice(h->device));
   ShardState* sh = new ShardState();
@@ -437,7 +437,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   auto seg_default = [&](size_t total) { return nranks == 1 ? total : std::min(total, 2 * total / (size_t)nranks + 4096); };
   const size_t Kseg = seg_keys ? std::min(seg_keys, max_nnz) : seg_default(max_nnz);
   const size_t Nseg = seg_nnz ? std::min(seg_nnz, max_nnz) : seg_default(max_nnz);
-  sh->lay.compute(nranks, K, max_rows, Kseg, Nseg);
+  sh->lay.compute(nranks, ks, max_rows, Kseg, Nseg);
   sh->timeout_cycles = h->shard_timeout_ms * 2000000LL;
   auto fail = [&](int rc) { dfbh::shard_destroy(h); return rc; };
   cudaError_t e;
@@ -463,7 +463,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
       (rc = h->ensure(sh->ws, (tot / 32 + 64) * 4)))
     return fail(rc);
   if (nranks > 1 && ((rc = h->ensure(sh->conf[0], tot)) || (rc = h->ensure(sh->conf[1], tot)) ||
-                     (rc = h->ensure(sh->vsave, tot * (size_t)K * 4))))
+                     (rc = h->ensure(sh->vsave, tot * (size_t)ks * 4))))
     return fail(rc);
   // Every workspace a step can touch is allocated NOW, for the declared capacities: a cudaMalloc / cudaFree in the
   // middle of a step is not just slow -- with peer access enabled it synchronises the peer devices, whose pollers

@@ -11,9 +11,10 @@
 //     cstart   i32 [Kseg+1]                     CSC column offsets of those keys (row lists in occ)
 //     occ      u32|u64 [Nseg]                   per column: the rows that contain it, in row order (+ value bits)
 //     rowptr   u64 [Bcap+1], ridx u32 [Nseg], rval f32 [Nseg]    the same non-zeros as a CSR over the worker's rows
-//     p        f32 [Bcap], pxv f32 [Bcap][K]    after the worker's reduce: p_i and p_i * XV_i   (fm_loss.h:155-195)
+//     p        f32 [Bcap], pxv f32 [Bcap][ks]   after the worker's reduce: p_i and p_i * XV_i   (fm_loss.h:155-195)
 //   written by owner s into worker r's mailbox, slot [parity][s]:
-//     part_xv  f32 [Bcap][K], part_sc float2 [Bcap]     partial XV / {sum (xV)^2, sum x w} over s's keys
+//     part_xv  f32 [Bcap][ks], part_sc float2 [Bcap]    partial XV / {sum (xV)^2, sum x w} over s's keys
+//   (ks = V_dim rounded up to 4 floats, the stride of the table rows)
 //     pen      f64                                       penalty of the weights r "pulled" from s (sgd_learner.cc:249-273)
 //   step counters (u64, one 64-byte line each): f_struct[r], f_pxv[r] (worker r -> me as owner),
 //                                               f_part[s], f_done[s] (owner s -> me as worker)
@@ -31,7 +32,7 @@ struct ShardBounds {
 };
 
 struct ShardLayout {
-  int S = 1, K = 0;
+  int S = 1, ks = 0;
   size_t Bcap = 0, Kseg = 0, Nseg = 0;
   size_t off_hdr = 0, off_keys = 0, off_cstart = 0, off_occ = 0, off_rowptr = 0, off_ridx = 0, off_rval = 0,
          off_p = 0, off_pxv = 0, off_part_xv = 0, off_part_sc = 0, off_pen = 0, off_flags = 0, total = 0;
@@ -46,8 +47,8 @@ struct ShardLayout {
     return reinterpret_cast<unsigned long long*>(static_cast<char*>(base) + off_flags + ((size_t)kind * 8 + i) * 64);
   }
   static size_t al(size_t n) { return (n + 255) / 256 * 256; }
-  void compute(int S_, int K_, size_t Bcap_, size_t Kseg_, size_t Nseg_) {
-    S = S_; K = K_; Bcap = Bcap_; Kseg = Kseg_; Nseg = Nseg_;
+  void compute(int S_, int ks_, size_t Bcap_, size_t Kseg_, size_t Nseg_) {
+    S = S_; ks = ks_; Bcap = Bcap_; Kseg = Kseg_; Nseg = Nseg_;
     size_t o = 0;
     auto region = [&](size_t& off, size_t& str, size_t bytes) { off = o; str = al(bytes); o += 2 * (size_t)S * str; };
     region(off_hdr, str_hdr, sizeof(ShardHdr));
@@ -58,8 +59,8 @@ struct ShardLayout {
     region(off_ridx, str_ridx, Nseg * 4);
     region(off_rval, str_rval, Nseg * 4);
     region(off_p, str_p, Bcap * 4);
-    region(off_pxv, str_pxv, Bcap * (size_t)K * 4);
-    region(off_part_xv, str_part_xv, Bcap * (size_t)K * 4);
+    region(off_pxv, str_pxv, Bcap * (size_t)ks * 4);
+    region(off_part_xv, str_part_xv, Bcap * (size_t)ks * 4);
     region(off_part_sc, str_part_sc, Bcap * 8);
     region(off_pen, str_pen, 8);
     off_flags = o;
@@ -86,7 +87,7 @@ struct RowptrDst { uint64_t* rowptr_dst[8]; };
 struct FillDst { uint32_t* ridx_dst[8]; float* rval_dst[8]; };
 
 struct ReduceArgs {
-  int S, me, train;
+  int S, me, train, V_dim;
   size_t nrows;
   const ShardBounds* wb;       // !wb->valid: the batch was dropped, the owners computed no partials for it
   const float* part_xv[8];
@@ -120,10 +121,10 @@ int launch_shard_scatter(const ScatterArgs& a, bool valued, size_t work_cap, cud
 int launch_shard_subcsr(const uint64_t* offset, const uint32_t* lidx, const float* value, size_t nrows,
                         const ShardBounds* wb, int S, int* rowcnt, const RowptrDst& rd, const FillDst& fd,
                         cudaStream_t s);
-int launch_shard_reduce(int V_dim, const ReduceArgs& a, cudaStream_t s);
-// one launch per worker, in rank order (conf / vsave: [S][Kseg] flags and [S][Kseg][K] saved rows; unused when stamp == 0)
+int launch_shard_reduce(const ReduceArgs& a, cudaStream_t s);
+// one launch per worker, in rank order (conf / vsave: [S][Kseg] flags and [S][Kseg][ks] saved rows; unused when stamp == 0)
 int launch_shard_lookup(Table& t, const LookupArgs& a, int r, bool insert, unsigned char* conf, cudaStream_t s);
-int launch_shard_pull(Table& t, const LookupArgs& a, const unsigned char* conf, float* vsave, int K, cudaStream_t s);
+int launch_shard_pull(Table& t, const LookupArgs& a, const unsigned char* conf, float* vsave, cudaStream_t s);
 int launch_shard_done(DevProgress* src_prog, DevProgress* main_prog, double* pen_dst, unsigned long long* flag_dst,
                       unsigned long long value, cudaStream_t s);
 int launch_shard_collect(const double* pen_in, int stride_f64, int S, DevProgress* prog_w, DevProgress* main_prog,

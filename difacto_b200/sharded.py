@@ -330,7 +330,9 @@ class FusedShardedStore:
     on their owner: owners compute the partial FM interaction sums of every worker's rows and ship (k+2) floats
     per EXAMPLE; the whole protocol (GPU localizer, slicing, peer stores, step-counter flags) runs on the
     device.  This class only does the plumbing a host has to do once: exchange the mailbox handles (CUDA IPC,
-    one process per GPU) through torch.distributed, or wire engines of the same process together."""
+    one process per GPU) through torch.distributed, or wire engines of the same process together.
+    Serves every 0 <= V_dim <= 128 with scatter=sorted (dfb_shard_init refuses other configurations: use
+    ShardedStore for them)."""
 
     def __init__(self, engine, max_rows, max_nnz, group=None, seg_keys=0, seg_nnz=0):
         self.E = engine

@@ -94,7 +94,8 @@ typedef struct {
  *                         chunks by separate warps, then finished in chunk order (0: one warp per key)
  *   long_row_nnz (1024)   an example with at least this many nonzeros is walked by a whole CTA in the forward
  *                         kernel, its chunks added in a fixed order (0: one warp per example whatever its length)
- *   force_generic (0)     1 = use the any-V_dim kernels even where a specialised one exists (tests)
+ *   force_generic (0)     1 = use the any-V_dim kernels even where a specialised one exists (tests).  Specialised
+ *                         kernels exist for 0 <= V_dim <= 128 (the atomic scatter: V_dim in {8,16,32,64,128})
  * Keys that are neither are returned through dfb_unknown_kwarg, mirroring the
  * "return the unconsumed kwargs" convention (updater.h:34, main.cc:25-31).
  * ------------------------------------------------------------------------------- */
@@ -327,7 +328,8 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
  * each taken at the V the worker "pulled" at step start.  What crosses NVLink is not the k-wide rows but the
  * per-example partial interaction sums (see csrc/kernels_shard.cu); nothing is synchronised with the host.
  *   dfb_shard_init     allocate this rank's mailbox (capacity: max_rows x max_nnz per minibatch; seg_keys /
- *                      seg_nnz = capacity of one (worker, owner) key segment, 0 = twice the even share)
+ *                      seg_nnz = capacity of one (worker, owner) key segment, 0 = twice the even share).  Needs
+ *                      0 <= V_dim <= 128, scatter=sorted and force_generic=0 (DFB_ERR_INVALID otherwise)
  *   dfb_shard_export   the mailbox pointer (peers in the same process) and its CUDA IPC handle (peers in
  *                      other processes open it with dfb_peer_open)
  *   dfb_shard_connect  the peers' mailbox pointers, indexed by rank (entry [rank] is ignored)
