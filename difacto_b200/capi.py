@@ -35,11 +35,17 @@ EXPORTS = [
     "dfb_peer_alloc", "dfb_peer_open", "dfb_peer_close", "dfb_peer_free", "dfb_dev_pull_rows_peer",
     "dfb_dev_fm_step_peer", "dfb_localize", "dfb_train_step_raw", "dfb_train_step_raw_async",
     "dfb_train_step_raw_dev", "dfb_prefetch_raw", "dfb_snapshot_size", "dfb_snapshot", "dfb_restore",
+    "dfb_snapshot_write", "dfb_restore_read",
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
 ]
 
 _LIB = None
+
+# dfb_write_fn / dfb_read_fn of the streamed checkpoint
+WRITE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t)
+READ_FN = C.CFUNCTYPE(C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t)
+READ_ERROR = 2 ** 64 - 1     # (size_t)-1
 
 
 def lib():
@@ -100,6 +106,9 @@ def lib():
         L.dfb_snapshot_size.argtypes = [vp, C.c_int, C.POINTER(sz)]
         L.dfb_snapshot.argtypes = [vp, C.c_int, vp, sz]
         L.dfb_restore.argtypes = [vp, vp, sz, C.POINTER(C.c_int)]
+        L.dfb_snapshot_write.argtypes = [vp, C.c_int, sz, WRITE_FN, vp]
+        L.dfb_restore_read.argtypes = [vp, READ_FN, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, sz,
+                                       C.POINTER(C.c_int)]
         L.dfb_shard_init.argtypes = [vp, C.c_int, C.c_int, sz, sz, sz, sz, C.POINTER(sz)]
         L.dfb_shard_export.argtypes = [vp, C.POINTER(vp), vp]
         L.dfb_shard_connect.argtypes = [vp, vp]
@@ -357,12 +366,51 @@ class Engine:
         self._ck(self.L.dfb_snapshot_size(self.h, int(save_aux), C.byref(n)))
         buf = (C.c_ubyte * max(n.value, 1))()
         self._ck(self.L.dfb_snapshot(self.h, int(save_aux), buf, n.value))
-        return bytes(buf[:n.value])
+        return C.string_at(buf, n.value)
 
     def restore(self, blob):
         buf = (C.c_ubyte * len(blob)).from_buffer_copy(blob)
         aux = C.c_int()
         self._ck(self.L.dfb_restore(self.h, buf, len(blob), C.byref(aux)))
+        return bool(aux.value)
+
+    def snapshot_to(self, fileobj, save_aux=True, chunk_bytes=0):
+        """stream the snapshot (dfb_snapshot_write) into fileobj.write, at most chunk_bytes per call"""
+        failed = []
+
+        def write(_ctx, buf, n):
+            try:
+                fileobj.write(C.string_at(buf, n))
+                return 0
+            except Exception as e:     # reported after the C call returns
+                failed.append(e)
+                return 1
+        cb = WRITE_FN(write)
+        rc = self.L.dfb_snapshot_write(self.h, int(save_aux), int(chunk_bytes), cb, None)
+        if failed:
+            raise DfbError(rc, self.L.dfb_last_error(self.h).decode()) from failed[0]
+        self._ck(rc)
+
+    def restore_from(self, fileobj, part=0, nparts=1, shard=0, nshards=1, chunk_bytes=0):
+        """restore (merge) one snapshot stream read from fileobj.read (dfb_restore_read); returns has_aux"""
+        failed = []
+
+        def read(_ctx, buf, cap):
+            try:
+                data = fileobj.read(cap)
+                if len(data) > cap:
+                    raise ValueError("read returned more than asked for")
+                C.memmove(buf, data, len(data))
+                return len(data)
+            except Exception as e:
+                failed.append(e)
+                return READ_ERROR
+        cb = READ_FN(read)
+        aux = C.c_int()
+        rc = self.L.dfb_restore_read(self.h, cb, None, part, nparts, shard, nshards, int(chunk_bytes), C.byref(aux))
+        if failed:
+            raise DfbError(rc, self.L.dfb_last_error(self.h).decode()) from failed[0]
+        self._ck(rc)
         return bool(aux.value)
 
     def read_entries(self, keys):

@@ -279,6 +279,32 @@ int launch_restore(Table& t, const uint64_t* keys, size_t n, const float* scal, 
 int launch_read_entries(Table& t, const int* slot, size_t n, float* scal, int* hasv, float* V,
                         float* cg, int k, cudaStream_t s);
 
+// ---- streamed checkpoint (kernels_checkpoint.cu, host side in checkpoint.cu) ----
+// the writer histograms the table by the top kCkptBinBits bits of the reversed key: [2^20] keys and V rows per bin
+constexpr int kCkptBinBits = 20;
+// DevProgress::err codes of the reader, mapped to messages by checkpoint.cu (the table is cleared on either)
+constexpr int kErrCkptDup = -101;     // a restored key was already in the table
+constexpr int kErrCkptRange = -102;   // a key outside the declared source part's range
+// the workspace of one writer pass of n records
+struct CkptWs {
+  unsigned long long *keys_in, *keys_out, *counter;
+  unsigned *slots_in, *slots_out, *hv, *vbefore;
+  void* tmp;
+  size_t tmp_bytes;
+  unsigned* out;      // the pass's packed records
+};
+int launch_ckpt_hist(const Table& t, unsigned* nk, unsigned* nv, cudaStream_t s);
+size_t ckpt_sort_tmp_bytes(size_t n);
+// the v1 records of the keys whose bin lies in [b0, b1) (n of them), in ascending key order, packed into ws.out
+int launch_ckpt_pass(const Table& t, unsigned b0, unsigned b1, size_t n, int aux, int k, const CkptWs& ws,
+                     cudaStream_t s);
+size_t rst_scan_tmp_bytes(size_t n);
+// n records of a chunk (roff: word offset of each record in buf): keep this shard's keys and insert them
+int launch_rst_chunk(Table& t, const unsigned* buf, const unsigned* roff, size_t n, int aux, int k, unsigned part,
+                     unsigned nparts, unsigned shard, unsigned nshards, unsigned long long* flags,
+                     unsigned long long* rank, void* tmp, size_t tmp_bytes, cudaStream_t s);
+int launch_rst_seed(Table& t, unsigned seed, cudaStream_t s);
+
 // ---- GPU localizer (kernels_localize.cu): Localizer::Compact + the CSC view from one radix sort ----
 size_t localize_sort_tmp_bytes(size_t nnz);
 // hi32: sort on the upper 32 key bits only (the caller knows the lower 32 are zero: ids < 2^32); verified on the device

@@ -1247,135 +1247,6 @@ int dfb_train_step(dfb_handle h, size_t nrows, const uint64_t* offset, const uin
   return dfb_read_progress(h, out);
 }
 
-// ------------------------------------------------------------------------------------------
-// checkpoint: Updater::Save / Load (include/difacto/updater.h:40-47; TODO stubs in the reference's
-// SGDUpdater, sgd_updater.h:44-50, so the byte format is ours)
-//   header { char magic[8] "DFB200\0\1"; u32 version; i32 V_dim; u64 n_keys; u64 n_vrows; u32 seed; u32 has_aux }
-//   n_keys records in ascending key order:
-//     u64 key; f32 fea_cnt; f32 w; [aux: f32 sqrt_g; f32 z;] i32 has_V; has_V ? f32 V[V_dim] [aux: f32 cg[V_dim]]
-// ------------------------------------------------------------------------------------------
-namespace {
-struct SnapHeader {
-  char magic[8];
-  uint32_t version;
-  int32_t V_dim;
-  uint64_t n_keys, n_vrows;
-  uint32_t seed, has_aux;
-};
-const char kSnapMagic[8] = {'D', 'F', 'B', '2', '0', '0', 0, 1};
-
-int snapshot_collect(dfb_engine* h, std::vector<Entry>* used, std::vector<float>* rows, TableState* st) {
-  DFB_CUDA(h, cudaStreamSynchronize(h->stream));
-  DFB_CUDA(h, cudaMemcpy(st, h->tab.state, sizeof(TableState), cudaMemcpyDeviceToHost));
-  std::vector<Entry> all(h->tab.cap);
-  DFB_CUDA(h, cudaMemcpy(all.data(), h->tab.tab, h->tab.cap * sizeof(Entry), cudaMemcpyDeviceToHost));
-  used->clear();
-  for (const Entry& e : all) if (e.key != kEmptyKey) used->push_back(e);
-  std::sort(used->begin(), used->end(), [](const Entry& a, const Entry& b) { return a.key < b.key; });
-  rows->resize((size_t)st->n_vrows * h->tab.rs);
-  if (!rows->empty())
-    DFB_CUDA(h, cudaMemcpy(rows->data(), h->tab.V, rows->size() * sizeof(float), cudaMemcpyDeviceToHost));
-  return 0;
-}
-}  // namespace
-
-int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes) {
-  if (!h || !bytes) return DFB_ERR_INVALID;
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  TableState st;
-  DFB_CUDA(h, cudaStreamSynchronize(h->stream));
-  DFB_CUDA(h, cudaMemcpy(&st, h->tab.state, sizeof(st), cudaMemcpyDeviceToHost));
-  const size_t k = (size_t)h->prm.V_dim;
-  *bytes = sizeof(SnapHeader) + st.n_keys * (8 + 8 + 4 + (save_aux ? 8 : 0)) + st.n_vrows * k * 4 * (save_aux ? 2 : 1);
-  return DFB_OK;
-}
-
-int dfb_snapshot(dfb_handle h, int save_aux, void* buf, size_t bytes) {
-  if (!h || !buf) return DFB_ERR_INVALID;
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  if (save_aux && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data to save");
-  std::vector<Entry> used;
-  std::vector<float> rows;
-  TableState st;
-  DFB_TRY(snapshot_collect(h, &used, &rows, &st));
-  const int k = h->prm.V_dim;
-  size_t need = 0;
-  DFB_TRY(dfb_snapshot_size(h, save_aux, &need));
-  if (bytes < need) return h->fail(DFB_ERR_INVALID, "snapshot buffer too small");
-  if (used.size() != st.n_keys) return h->fail(DFB_ERR_INVALID, "table changed while taking the snapshot");
-  char* p = static_cast<char*>(buf);
-  SnapHeader hd;
-  memcpy(hd.magic, kSnapMagic, 8);
-  hd.version = 1; hd.V_dim = k; hd.n_keys = st.n_keys; hd.n_vrows = st.n_vrows; hd.seed = st.seed;
-  hd.has_aux = save_aux ? 1 : 0;
-  memcpy(p, &hd, sizeof(hd)); p += sizeof(hd);
-  auto put = [&](const void* src, size_t n) { memcpy(p, src, n); p += n; };
-  for (const Entry& e : used) {
-    put(&e.key, 8); put(&e.fea_cnt, 4); put(&e.w, 4);
-    if (save_aux) { put(&e.sqrt_g, 4); put(&e.z, 4); }
-    const int32_t hv = e.vrow >= 0 ? 1 : 0;
-    put(&hv, 4);
-    if (hv) {
-      const float* r = rows.data() + (size_t)e.vrow * h->tab.rs;
-      put(r, (size_t)k * 4);
-      if (save_aux) put(r + h->tab.ks, (size_t)k * 4);
-    }
-  }
-  return DFB_OK;
-}
-
-int dfb_restore(dfb_handle h, const void* buf, size_t bytes, int* has_aux) {
-  if (!h || !buf) return DFB_ERR_INVALID;
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  if (bytes < sizeof(SnapHeader)) return h->fail(DFB_ERR_INVALID, "snapshot truncated");
-  const char* p = static_cast<const char*>(buf);
-  const char* end = p + bytes;
-  SnapHeader hd;
-  memcpy(&hd, p, sizeof(hd)); p += sizeof(hd);
-  if (memcmp(hd.magic, kSnapMagic, 8) != 0 || hd.version != 1) return h->fail(DFB_ERR_INVALID, "not a difacto_b200 snapshot");
-  if (hd.V_dim != h->prm.V_dim) return h->fail(DFB_ERR_INVALID, "snapshot V_dim differs from the engine's V_dim");
-  TableState st;
-  DFB_CUDA(h, cudaStreamSynchronize(h->stream));
-  DFB_CUDA(h, cudaMemcpy(&st, h->tab.state, sizeof(st), cudaMemcpyDeviceToHost));
-  if (st.n_keys != 0) return h->fail(DFB_ERR_INVALID, "dfb_restore needs an empty table");
-  if (hd.n_keys > h->tab.max_keys || hd.n_vrows > h->tab.vcap) return h->fail(DFB_ERR_CAPACITY, "snapshot larger than table_capacity / V_capacity");
-  const int k = hd.V_dim;
-  const bool aux = hd.has_aux != 0;
-  std::vector<uint64_t> keys(hd.n_keys);
-  std::vector<float> scal(hd.n_keys * 4, 0.f);
-  std::vector<int> vrow(hd.n_keys, -1);
-  std::vector<float> rows((size_t)hd.n_vrows * h->tab.rs, 0.f);
-  uint64_t nv = 0;
-  auto get = [&](void* dst, size_t n) { if (p + n > end) return false; memcpy(dst, p, n); p += n; return true; };
-  for (uint64_t i = 0; i < hd.n_keys; ++i) {
-    bool ok = get(&keys[i], 8) && get(&scal[i * 4 + 0], 4) && get(&scal[i * 4 + 1], 4);
-    if (ok && aux) ok = get(&scal[i * 4 + 2], 4) && get(&scal[i * 4 + 3], 4);
-    int32_t hv = 0;
-    ok = ok && get(&hv, 4);
-    if (ok && hv) {
-      if (nv >= hd.n_vrows) return h->fail(DFB_ERR_INVALID, "snapshot corrupt (V rows)");
-      float* r = rows.data() + (size_t)nv * h->tab.rs;
-      ok = get(r, (size_t)k * 4);
-      if (ok && aux) ok = get(r + h->tab.ks, (size_t)k * 4);
-      vrow[i] = (int)nv++;
-    }
-    if (!ok) return h->fail(DFB_ERR_INVALID, "snapshot truncated");
-  }
-  cudaStream_t s = h->stream;
-  DFB_TRY(h2d(h, h->keys, keys.data(), keys.size() * 8, s));
-  DFB_TRY(h2d(h, h->scal, scal.data(), scal.size() * 4, s));
-  DFB_TRY(h2d(h, h->hasv, vrow.data(), vrow.size() * 4, s));
-  if (!rows.empty()) DFB_CUDA(h, cudaMemcpyAsync(h->tab.V, rows.data(), rows.size() * 4, cudaMemcpyHostToDevice, s));
-  h->launches += launch_restore(h->tab, h->keys.as<uint64_t>(), keys.size(), h->scal.as<float>(), h->hasv.as<int>(),
-                                nv, hd.seed, s);
-  DFB_TRY(sync_and_check(h));
-  DFB_CUDA(h, cudaMemsetAsync(h->tab.prog, 0, sizeof(DevProgress), s));   // restoring is not "new keys" of a step
-  DFB_CUDA(h, cudaStreamSynchronize(s));
-  h->has_aux = aux ? 1 : 0;
-  if (has_aux) *has_aux = h->has_aux;
-  return DFB_OK;
-}
-
 int dfb_read_entries(dfb_handle h, const uint64_t* keys, size_t n, float* scal_out, int* has_V_out, float* V_out,
                      float* cg_out) {
   if (!h) return DFB_ERR_INVALID;

@@ -26,6 +26,7 @@ struct dfb_engine {
   int scatter_sorted = 1;   // 1: atomic-free sorted reduction (deterministic); 0: red.global atomics
   int overlap_auc = 1;      // run the AUC kernels on the auxiliary stream, concurrently with the update
   int has_aux = 1;          // false after restoring a snapshot saved without aux data (sgd_updater.h:88)
+  int restored_parts = 0;   // snapshot streams merged into the table since it was last empty (checkpoint.cu)
   int l2_hints = 1;         // per-load L2 eviction policies in the gather kernels
   int id_bits = 0;          // > 0: feature ids are < 2^id_bits (fixes the radix-sort bit range of the GPU localizer)
   int loc_begin_bit = -1;   // auto mode: lowest significant bit of the reversed keys seen so far (sticky)

@@ -48,6 +48,34 @@ class GpuEngine {
   KWArgs remain_;
 };
 
+/** the streamed checkpoint over std::ostream / std::istream (dfb_snapshot_write / dfb_restore_read) */
+inline int OstreamSink(void* ctx, const void* buf, size_t bytes) {
+  auto* fo = static_cast<std::ostream*>(ctx);
+  fo->write(static_cast<const char*>(buf), static_cast<std::streamsize>(bytes));
+  return fo->good() ? 0 : 1;
+}
+inline size_t IstreamSource(void* ctx, void* buf, size_t cap) {
+  auto* fi = static_cast<std::istream*>(ctx);
+  if (fi->bad()) return static_cast<size_t>(-1);
+  if (fi->eof()) return 0;
+  fi->read(static_cast<char*>(buf), static_cast<std::streamsize>(cap));
+  if (fi->bad()) return static_cast<size_t>(-1);
+  return static_cast<size_t>(fi->gcount());
+}
+/** save engine e's model to fo, one chunk at a time */
+inline void SaveEngine(const GpuEngine& e, bool save_aux, std::ostream* fo) {
+  e.Check(dfb_snapshot_write(e.handle(), save_aux ? 1 : 0, 0, OstreamSink, fo), "dfb_snapshot_write");
+  fo->flush();
+  if (!fo->good()) throw Error("failed to write the model");
+}
+/** restore (merge) part `part` of `nparts` read from fi into engine e, shard `shard` of `nshards`; returns has_aux */
+inline bool RestoreEngine(const GpuEngine& e, std::istream* fi, uint32_t part, uint32_t nparts, uint32_t shard,
+                          uint32_t nshards) {
+  int aux = 0;
+  e.Check(dfb_restore_read(e.handle(), IstreamSource, fi, part, nparts, shard, nshards, 0, &aux), "dfb_restore_read");
+  return aux != 0;
+}
+
 /** the reference's SGDUpdaterParam fields the host needs to see (src/sgd/sgd_param.h:66-107) */
 struct SGDUpdaterParamView {
   float l1 = 1, l2 = 0, V_l2 = .01f;
@@ -67,20 +95,16 @@ class GpuSGDUpdater : public Updater {
     return engine_->remain();
   }
   /** Updater::Load / Save (updater.h:40-47).  TODO stubs in the reference's SGDUpdater
-   * (sgd_updater.h:44-50); here a snapshot of the table in the format of dfb_snapshot. */
+   * (sgd_updater.h:44-50); here a snapshot of the table in the format of dfb_snapshot, streamed through the GPU
+   * in bounded host memory.  Load needs an empty table, like dfb_restore. */
   void Load(std::istream* fi, bool* has_aux) override {
-    std::string blob((std::istreambuf_iterator<char>(*fi)), std::istreambuf_iterator<char>());
-    int aux = 0;
-    engine_->Check(dfb_restore(engine_->handle(), blob.data(), blob.size(), &aux), "dfb_restore");
-    if (has_aux) *has_aux = aux != 0;
+    uint64_t n_keys = 0;
+    engine_->Check(dfb_table_stats(engine_->handle(), &n_keys, nullptr, nullptr, nullptr), "dfb_table_stats");
+    if (n_keys != 0) throw Error("Load needs an empty table");
+    const bool aux = RestoreEngine(*engine_, fi, 0, 1, 0, 1);
+    if (has_aux) *has_aux = aux;
   }
-  void Save(bool save_aux, std::ostream* fo) const override {
-    size_t n = 0;
-    engine_->Check(dfb_snapshot_size(engine_->handle(), save_aux ? 1 : 0, &n), "dfb_snapshot_size");
-    std::string blob(n, '\0');
-    engine_->Check(dfb_snapshot(engine_->handle(), save_aux ? 1 : 0, &blob[0], n), "dfb_snapshot");
-    fo->write(blob.data(), static_cast<std::streamsize>(n));
-  }
+  void Save(bool save_aux, std::ostream* fo) const override { SaveEngine(*engine_, save_aux, fo); }
 
   /** SGDUpdater::Get, sgd_updater.cc:32-56 */
   void Get(const SArray<feaid_t>& fea_ids, int val_type, SArray<real_t>* weights, SArray<int>* lens) override {

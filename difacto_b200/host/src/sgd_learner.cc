@@ -2,6 +2,7 @@
 // src/sgd/sgd_learner.cc of the reference (cited per function); the arithmetic lives on the GPU.
 #include "difacto_b200/sgd_learner.h"
 
+#include <cstdint>
 #include <cstdio>
 #include <fstream>
 #include <thread>
@@ -63,16 +64,53 @@ KWArgs SGDLearner::Init(const KWArgs& kwargs) {
   return remain;
 }
 
-// model_in -> the engine(s): one file, or <name>_part-<r> per shard when num_gpus = N > 1
+namespace {
+bool FileExists(const std::string& fn) { return static_cast<bool>(std::ifstream(fn, std::ios::binary)); }
+
+// ps-lite's key range of shard r of S (postoffice.cc:127-136; the tail above UINT64_MAX/S*S belongs to S-1), as
+// an inclusive [lo, hi]
+void KeyRange(uint32_t r, uint32_t S, uint64_t* lo, uint64_t* hi) {
+  const uint64_t width = UINT64_MAX / S;
+  *lo = width * r;
+  *hi = r + 1 == S ? UINT64_MAX : width * (r + 1) - 1;
+}
+}  // namespace
+
+// model_in = X -> the engine(s).  The model is one file X (a num_gpus = 1 run) or the parts X_part-0 .. X_part-(M-1)
+// of a num_gpus = M run.  num_gpus = 1 reads X when it exists, otherwise the parts; num_gpus = N > 1 reads the parts
+// when X_part-0 exists, otherwise X.  Rank r of N restores every part whose key range overlaps its own and keeps its
+// keys (dfb_restore_read), so M parts load into any number of GPUs; M = N is part r alone.
 void SGDLearner::LoadShards() {
-  for (int r = 0; r < param_.num_gpus; ++r) {
-    const std::string fn = param_.num_gpus > 1 ? param_.model_in + "_part-" + std::to_string(r) : param_.model_in;
-    std::ifstream fi(fn, std::ios::binary);
-    if (!fi) throw Error("failed to open model_in " + fn);
-    std::string blob((std::istreambuf_iterator<char>(fi)), std::istreambuf_iterator<char>());
-    int aux = 0;
-    ShardEngine(r)->Check(dfb_restore(ShardEngine(r)->handle(), blob.data(), blob.size(), &aux), "dfb_restore");
-    if (verbose) printf("Loaded model from %s (%s aux data)\n", fn.c_str(), aux ? "with" : "without");
+  const std::string& base = param_.model_in;
+  auto part_name = [&](int p) { return base + "_part-" + std::to_string(p); };
+  const bool parts = param_.num_gpus > 1 ? FileExists(part_name(0)) : !FileExists(base);
+  std::vector<std::string> files;
+  if (parts) {
+    for (int p = 0; FileExists(part_name(p)); ++p) files.push_back(part_name(p));
+  } else if (FileExists(base)) {
+    files.push_back(base);
+  }
+  if (files.empty()) throw Error("failed to open model_in " + base + " (nor " + part_name(0) + ")");
+  const uint32_t M = static_cast<uint32_t>(files.size()), N = static_cast<uint32_t>(param_.num_gpus);
+  for (uint32_t r = 0; r < N; ++r) {
+    uint64_t rlo, rhi;
+    KeyRange(r, N, &rlo, &rhi);
+    bool aux = true;
+    int read = 0;
+    for (uint32_t p = 0; p < M; ++p) {
+      uint64_t plo, phi;
+      KeyRange(p, M, &plo, &phi);
+      if (plo > rhi || rlo > phi) continue;      // part p cannot hold keys of rank r
+      std::ifstream fi(files[p], std::ios::binary);
+      if (!fi) throw Error("failed to open model_in " + files[p]);
+      aux = RestoreEngine(*ShardEngine(r), &fi, p, M, r, N) && aux;
+      ++read;
+    }
+    if (verbose) {
+      printf("Loaded model from %s (%u part%s", base.c_str(), M, M > 1 ? "s" : "");
+      if (N > 1) printf(", %d read by GPU %u", read, r);
+      printf(", %s aux data)\n", aux ? "with" : "without");
+    }
   }
 }
 
@@ -88,11 +126,7 @@ void SGDLearner::RunScheduler() {
       const std::string fn = shard_name(param_.model_out, r);
       std::ofstream fo(fn, std::ios::binary);
       if (!fo) throw Error("failed to open model_out " + fn);
-      size_t n = 0;
-      ShardEngine(r)->Check(dfb_snapshot_size(ShardEngine(r)->handle(), 1, &n), "dfb_snapshot_size");
-      std::string blob(n, '\0');
-      ShardEngine(r)->Check(dfb_snapshot(ShardEngine(r)->handle(), 1, &blob[0], n), "dfb_snapshot");
-      fo.write(blob.data(), static_cast<std::streamsize>(n));
+      SaveEngine(*ShardEngine(r), true, &fo);
       if (verbose) printf("Saved model to %s\n", fn.c_str());
     }
   }
@@ -101,8 +135,8 @@ void SGDLearner::RunScheduler() {
 sgd::Progress SGDLearner::Predict() {
   if (param_.model_in.empty()) throw Error("task=predict needs model_in");
   if (param_.num_gpus > 1) {
-    // the shards of a num_gpus = N run, scored by the same N GPUs (loss / AUC only: the rows of a step are spread
-    // over the workers, so there is no single prediction file to write)
+    // the model (one file or any number of parts), re-sharded over and scored by N GPUs (loss / AUC only: the rows
+    // of a step are spread over the workers, so there is no single prediction file to write)
     if (!param_.pred_out.empty()) throw Error("pred_out needs num_gpus=1 (the predictions of a sharded run are spread over the workers)");
     LoadShards();
     sgd::Progress prog;
@@ -111,10 +145,7 @@ sgd::Progress SGDLearner::Predict() {
     if (verbose) printf(" - Prediction: %s, rows = %g\n", prog.TextString().c_str(), prog.nrows);
     return prog;
   }
-  std::ifstream fi(param_.model_in, std::ios::binary);
-  if (!fi) throw Error("failed to open model_in " + param_.model_in);
-  bool has_aux = false;
-  GetUpdater()->Load(&fi, &has_aux);
+  LoadShards();      // one file, or all parts of a num_gpus = M model merged into this GPU
   FILE* fo = param_.pred_out.empty() ? nullptr : fopen(param_.pred_out.c_str(), "w");
   if (!param_.pred_out.empty() && !fo) throw Error("failed to open pred_out " + param_.pred_out);
   sgd::Progress prog;

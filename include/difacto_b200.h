@@ -252,11 +252,38 @@ int dfb_profile_read(dfb_handle h, double* stage_ms, uint64_t* stage_count);
 int dfb_read_entries(dfb_handle h, const uint64_t* keys, size_t n, float* scal_out,
                      int* has_V_out, float* V_out, float* cg_out);
 /* checkpoint = Updater::Save / Updater::Load (include/difacto/updater.h:40-47; TODO stubs in the
- * reference's SGDUpdater, sgd_updater.h:44-50, so the byte format is this library's: header +
- * records in ascending key order {key, fea_cnt, w, [sqrt_g, z], has_V, V[V_dim], [cg[V_dim]]}, the
- * bracketed fields only with save_aux).  dfb_restore needs an empty table with the same V_dim; a
- * snapshot without aux data restores a model that can predict but not train ("no aux data",
- * sgd_updater.cc:75). */
+ * reference's SGDUpdater, sgd_updater.h:44-50, so the byte format is this library's).  Format v1, little-endian:
+ *   header (40 bytes) { char magic[8] = "DFB200\0\1"; u32 version = 1; i32 V_dim; u64 n_keys; u64 n_vrows;
+ *                       u32 seed (the InitV rand_r state); u32 has_aux }
+ *   n_keys records in strictly ascending (reversed) key order:
+ *     { u64 key; f32 fea_cnt; f32 w; [f32 sqrt_g; f32 z;] i32 has_V (0/1); has_V: f32 V[V_dim] [f32 cg[V_dim]] }
+ *   the bracketed fields only with save_aux.  A snapshot without aux data restores a model that can predict but
+ *   not train ("no aux data", sgd_updater.cc:75).
+ * Streaming: dfb_snapshot_write sorts and packs the records on the device and hands the stream to write_fn in
+ * pieces of at most chunk_bytes (0 = 64 MiB; at least 40); host memory is two pinned chunks and an 8 MB
+ * histogram, device workspace is allocated for the call (about 4 x chunk_bytes of records, more when the keys
+ * that share their top 20 bits need more) and released at its end.  dfb_restore_read pulls the stream from
+ * read_fn in chunks of at most chunk_bytes (0 = 64 MiB), validates it on the host (magic, version, V_dim, has_V,
+ * ascending keys, truncation, the header's counts) and unpacks it on the device.  Both wait for every stream of
+ * the handle first: they run between steps, never while steps are in flight.
+ * Re-sharding: the stream is part `part` of `nparts` (a num_gpus = nparts run's rank `part`, or 0 of 1); the engine
+ * is shard `shard` of `nshards` and keeps the keys with dfb_key_owner(key, nshards) == shard.  A key outside the
+ * part's own ps-lite range is DFB_ERR_INVALID (parts miscounted or mixed up).  Several calls merge several parts
+ * into one engine; a key restored twice is DFB_ERR_INVALID.  V rows are appended in stream order.
+ * Seed and aux: the InitV state comes from the header of the first stream restored into an empty table, so an
+ * nparts == nshards restore gives every rank its own part's stream, exactly as it was saved; after a re-shard
+ * (nparts != nshards) each rank continues the InitV stream of the lowest part it read (a convention: the reference
+ * has no checkpoint to compare with).  has_aux is the AND over the streams restored.
+ * Errors: a failed dfb_restore_read (bad stream, capacity, read_fn error) leaves an EMPTY table behind -- the
+ * message says the table was cleared -- so that the caller can retry.  dfb_snapshot_write changes nothing, also
+ * when write_fn fails.
+ * dfb_snapshot / dfb_restore are the same over one memory buffer (dfb_snapshot_size bytes); dfb_restore needs an
+ * empty table (refused without clearing anything otherwise). */
+typedef int (*dfb_write_fn)(void* ctx, const void* buf, size_t bytes);   /* 0 = ok */
+typedef size_t (*dfb_read_fn)(void* ctx, void* buf, size_t cap);       /* bytes read, 0 = end, (size_t)-1 = error */
+int dfb_snapshot_write(dfb_handle h, int save_aux, size_t chunk_bytes, dfb_write_fn write_fn, void* ctx);
+int dfb_restore_read(dfb_handle h, dfb_read_fn read_fn, void* ctx, uint32_t part, uint32_t nparts, uint32_t shard,
+                     uint32_t nshards, size_t chunk_bytes, int* has_aux_out);
 int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes);
 int dfb_snapshot(dfb_handle h, int save_aux, void* buf, size_t bytes);
 int dfb_restore(dfb_handle h, const void* buf, size_t bytes, int* has_aux_out);
