@@ -38,6 +38,7 @@ EXPORTS = [
     "dfb_snapshot_write", "dfb_restore_read",
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
+    "dfb_predict_raw_async", "dfb_predict_raw_dev", "dfb_shard_predict_async", "dfb_shard_begin_predict_async",
 ]
 
 _LIB = None
@@ -119,6 +120,10 @@ def lib():
         L.dfb_shard_begin_async.argtypes = [vp, sz, vp, vp, vp, vp, C.c_int, C.c_int]
         L.dfb_shard_begin_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, C.c_int, C.c_int]
         L.dfb_shard_phase.argtypes = [vp, C.c_int]
+        L.dfb_predict_raw_async.argtypes = [vp, sz, vp, vp, vp, vp, vp]
+        L.dfb_predict_raw_dev.argtypes = [vp, sz, sz, vp, vp, vp, vp, vp]
+        L.dfb_shard_predict_async.argtypes = [vp, sz, vp, vp, vp, vp, vp]
+        L.dfb_shard_begin_predict_async.argtypes = [vp, sz, vp, vp, vp, vp, vp]
         L.dfb_shard_info.argtypes = [vp, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(sz), C.POINTER(sz),
                                      C.POINTER(u64)]
         L.dfb_stream.restype = vp
@@ -317,6 +322,25 @@ class Engine:
         self._ck(self.L.dfb_train_step_raw_dev(self.h, nrows, nnz, _p(d_offset), _p(d_ids), _p(d_value), _p(d_label),
                                                int(push_cnt), int(is_train)))
 
+    # ---- raw ids: predict steps (the forward pass of a frozen model; nothing of the model is written) ----
+    def predict_raw(self, offset, ids, value=None, label=None):
+        """one predict step, waited for: (Progress read as train_step_raw reads it, predictions[nrows])"""
+        offset, ids = _arr(offset, np.uint64), _arr(ids, np.uint64)
+        value, label = _arr(value, np.float32), _arr(label, np.float32)
+        nrows = len(offset) - 1
+        pred = np.zeros(max(nrows, 1), np.float32)
+        self.predict_raw_async(nrows, offset, ids, value, label, pred)
+        return self.read_progress(), pred[:nrows]
+
+    def predict_raw_async(self, nrows, offset, ids, value, label, pred_out):
+        """raw pointers / arrays, no conversion: pred_out (pinned for an asynchronous copy) is written when the step is
+        collected (wait_step / read_progress / sync)"""
+        self._ck(self.L.dfb_predict_raw_async(self.h, nrows, _p(offset), _p(ids), _p(value), _p(label), _p(pred_out)))
+
+    def predict_raw_dev(self, nrows, nnz, d_offset, d_ids, d_value, d_label, d_pred_out=None):
+        self._ck(self.L.dfb_predict_raw_dev(self.h, nrows, nnz, _p(d_offset), _p(d_ids), _p(d_value), _p(d_label),
+                                            _p(d_pred_out)))
+
     def train_step_async(self, nrows, offset, lidx, value, label, keys, nkeys, cnt=None, is_train=True):
         """raw pointers / arrays, no conversion: for pinned-memory pipelines"""
         self._ck(self.L.dfb_train_step_async(self.h, nrows, _p(offset), _p(lidx), _p(value), _p(label),
@@ -492,6 +516,14 @@ class Engine:
     def shard_begin_dev(self, nrows, nnz, d_offset, d_ids, d_value, d_label, push_cnt=False, is_train=True):
         self._ck(self.L.dfb_shard_begin_dev(self.h, nrows, nnz, _p(d_offset), _p(d_ids), _p(d_value), _p(d_label),
                                             int(push_cnt), int(is_train)))
+
+    def shard_predict_async(self, nrows, offset, ids, value, label, pred_out):
+        self._ck(self.L.dfb_shard_predict_async(self.h, nrows, _p(offset), _p(ids), _p(value), _p(label),
+                                                _p(pred_out)))
+
+    def shard_begin_predict_async(self, nrows, offset, ids, value, label, pred_out):
+        self._ck(self.L.dfb_shard_begin_predict_async(self.h, nrows, _p(offset), _p(ids), _p(value), _p(label),
+                                                      _p(pred_out)))
 
     def shard_phase(self, phase):
         self._ck(self.L.dfb_shard_phase(self.h, int(phase)))

@@ -19,6 +19,18 @@ __device__ __forceinline__ uint64_t hash64(uint64_t h) {
   return h;
 }
 
+__device__ __forceinline__ unsigned long long reverse_nibbles(unsigned long long x) {
+  // byte reversal, then swap the two nibbles of every byte  == reversing the 16 nibbles
+  x = ((unsigned long long)__byte_perm((unsigned)(x & 0xffffffffULL), 0, 0x0123) << 32) |
+      (unsigned long long)__byte_perm((unsigned)(x >> 32), 0, 0x0123);
+  return ((x & 0x0F0F0F0F0F0F0F0FULL) << 4) | ((x & 0xF0F0F0F0F0F0F0F0ULL) >> 4);
+}
+
+// the table key of a raw feature id as Localizer(-1) forms it: ReverseBytes(id % (2^64-1)) (localizer.cc:22-26)
+__device__ __forceinline__ unsigned long long raw_key(unsigned long long id) {
+  return reverse_nibbles(id == ~0ULL ? 0ULL : id);
+}
+
 __device__ __forceinline__ float warp_sum_f(float v) {
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFullMask, v, o);

@@ -90,6 +90,9 @@ struct FmView {
   int l2hint;
   // 1: the pulled view {w,vrow} is re-read per nnz and fits in L2 with room to spare (evict_last); 0: normal policy
   int wv_last;
+  // the raw-id forward (launch_fm_raw): the hash table that each nonzero's id is looked up in, find only
+  const Entry* tab;
+  unsigned long long tab_mask;
 };
 
 // where the worker's gradient rows go: locally contiguous (nseg == 0) or, per owner segment of the
@@ -179,6 +182,8 @@ struct FmBatch {
   // the localizer dropped the batch: the kernels then return at once, without reading the batch's ranks, and the
   // forward raises kErrIdRange into prog
   const unsigned long long* dev_nkeys;
+  // the raw feature id of every nnz (launch_fm_raw: replaces index)
+  const uint64_t* ids;
 };
 
 // true when the specialised (16-byte-lane) kernels serve this V_dim: 0 <= V_dim <= 128
@@ -217,6 +222,9 @@ size_t l2_bytes();
 // ---- launchers (kernels_fm.cu) ----
 // returns number of kernel launches performed, or <0 on invalid configuration
 int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s);
+// predict only, on raw ids (b.ids): the specialised kernels probe the table (v.tab) for each nonzero's key instead of
+// reading a pulled view; v.vbase / vstride = the table rows.  -1 when V_dim has no specialised kernels
+int launch_fm_raw(const FmBatch& b, const FmView& v, cudaStream_t s);
 // MODE 3: partial interaction sums of every source's rows (see PartArgs); v.vbase/vstride = the table rows
 int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s);
 int launch_grad_finalize(int V_dim, size_t nkeys, const float* weights, const int* V_pos,
@@ -319,6 +327,8 @@ int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_
                          DevProgress* prog /* nullptr: a dropped batch (n_unique = 0) is the caller's to report */,
                          cudaStream_t s);
 int launch_cnt_from_cols(const int* col_start, const int* col_end, size_t n, float* cnt, cudaStream_t s);
+// *ok (set non-zero by the caller) is cleared when an id of the n, mapped as Localizer(-1) maps it, is >= 2^nbits
+int launch_id_range(const uint64_t* ids, size_t n, int nbits, unsigned long long* ok, cudaStream_t s);
 
 // ---- sorted (atomic-free, deterministic) gradient reduction ----
 // CSC view of the batch: stable radix sort of (local key id -> occurrence payload); afterwards

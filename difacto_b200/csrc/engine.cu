@@ -215,10 +215,11 @@ int ensure_sorted_ws(dfb_engine* h, size_t nrows, size_t nnz, size_t U, bool val
 
 // U is the number of keys, or (dU != nullptr) the capacity of the key arrays with the actual count on the device
 // (a batch localized on the GPU never reports its size to the host); d_cnt / cnt_cols: see launch_feacnt.
+// predict: a predict step (dfb_predict_raw_* on widths without the raw-id kernels): no penalty; d_lab may be NULL.
 int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint32_t* d_idx,
              const float* d_val, const float* d_lab, const uint64_t* d_keys, size_t U, const float* d_cnt,
              int is_train, const dfb_engine::LocSet* csc = nullptr, const unsigned long long* dU = nullptr,
-             const int* cnt_cols = nullptr) {
+             const int* cnt_cols = nullptr, bool predict = false) {
   const bool csc_ready = csc != nullptr;
   const bool push_cnt = d_cnt != nullptr || cnt_cols != nullptr;
   if (U > 0x7fffffffULL || nrows > 0x7fffffffULL || nnz > 0x7fffffffULL)
@@ -302,7 +303,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     h->launches += nl;
   }
   bool auc_pending = false;
-  if (h->compute_auc && nrows) {
+  if (h->compute_auc && nrows && d_lab) {
     // AUC depends only on pred: run it on the auxiliary stream, overlapped with the gradient
     // reduction / update below (when profiling, keep it on the main stream so that it is timed)
     DFB_TRY(h->ensure(h->auc_k, nrows * sizeof(float)));
@@ -358,7 +359,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
                                        d_val ? h->gxxp.as<float>() : nullptr, h->gV.as<float>(), flags, 1,
                                        d_val ? 1 : 2, s);
     h->launches += launch_initv(h->tab, h->prm, slot, U, nullptr, flags, pos, s);
-  } else {
+  } else if (!predict) {
     h->launches += launch_penalty(h->prm, h->tab.prog, u_w, u_vrow, h->tab.V, h->tab.rs, 0, U, dU, s);
   }
   if (h->profile) {
@@ -483,7 +484,7 @@ namespace {
 // count stays on the device), so a step is one uninterrupted enqueue.
 int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                  const float* d_val, const float* d_lab, int push_cnt, int is_train, cudaEvent_t inputs_ready,
-                 bool exact_range = false) {
+                 bool exact_range = false, bool predict = false) {
   dfb_engine::LocSet& L = h->loc[h->loc_seq & 1];
   // while profiling the localizer shares the main stream: per-stage times are then those of kernels running alone
   cudaStream_t ls = h->profile ? h->stream : h->loc_stream;
@@ -516,12 +517,67 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
     h->launches += launch_raise_err(h->tab.prog, kErrIdRange, h->stream);
   } else {
     rc = step_dev(h, nrows, nnz, d_off, L.lidx.as<uint32_t>(), d_val, d_lab, L.keys.as<uint64_t>(), U, d_cnt,
-                  is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols);
+                  is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols, predict);
   }
   DFB_CUDA(h, cudaEventRecord(L.consumed, h->stream));
   L.used = true;
   h->loc_seq++;
   return rc;
+}
+
+// the predict step on raw ids: the forward pass of a frozen model, written into h->pred.  Nothing of the model is
+// written.  Where the specialised kernels exist it is ONE forward launch that probes the table for each nonzero's id
+// (no localizer, no key lookup, no penalty: launch_fm_raw), plus the id_bits range check when id_bits > 0 and the
+// AUC when labels are given.  Other widths (V_dim > 128, force_generic) run the validation step without its penalty.
+int predict_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
+                const float* d_val, const float* d_lab, cudaEvent_t inputs_ready) {
+  if (h->shard)
+    return h->fail(DFB_ERR_INVALID, "this engine holds one shard of a sharded model: predict with dfb_shard_predict_async");
+  if (nrows > 0x7fffffffULL || nnz > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "batch too large");
+  cudaStream_t s = h->stream;
+  DFB_TRY(h->ensure(h->pred, (nrows ? nrows : 1) * sizeof(float)));
+  if (!h->sorted_path(false)) {
+    // a dropped batch (ids outside id_bits) predicts 0 for every row
+    if (nrows) DFB_CUDA(h, cudaMemsetAsync(h->pred.p, 0, nrows * sizeof(float), s));
+    return step_raw_dev(h, nrows, nnz, d_off, d_ids, d_val, d_lab, 0, 0, inputs_ready, true, true);
+  }
+  if (h->profile && h->prof_steps && h->prof_steps % dfb_engine::kProfRing == 0) DFB_TRY(prof_drain(h));
+  FmView v;
+  memset(&v, 0, sizeof(v));
+  v.vbase = h->tab.V; v.vstride = h->tab.rs; v.l2hint = h->l2_hints;
+  v.tab = h->tab.tab; v.tab_mask = h->tab.mask;
+  FmBatch b;
+  memset(&b, 0, sizeof(b));
+  b.nrows = nrows; b.offset = d_off; b.ids = d_ids; b.value = d_val; b.label = d_lab;
+  b.pred_io = h->pred.as<float>(); b.V_dim = h->prm.V_dim; b.train = 0; b.prog = h->tab.prog;
+  b.long_nnz = (unsigned)h->long_row_nnz; b.nnz_hint = nnz;
+  const int nbits = 4 * ((h->id_bits + 3) / 4);
+  if (h->id_bits > 0 && nbits < 64 && nnz) {
+    // the range the localizer would sort: a batch outside it is dropped as a training batch would be (0 predictions,
+    // nothing in Progress, kErrIdRange raised by the forward kernel)
+    DFB_TRY(h->ensure(h->id_ok, sizeof(unsigned long long)));
+    DFB_CUDA(h, cudaMemsetAsync(h->id_ok.p, 0xff, sizeof(unsigned long long), s));
+    DFB_CUDA(h, cudaMemsetAsync(h->pred.p, 0, nrows * sizeof(float), s));
+    h->launches += launch_id_range(d_ids, nnz, nbits, h->id_ok.as<unsigned long long>(), s);
+    b.dev_nkeys = h->id_ok.as<unsigned long long>();
+  }
+  if (nrows) {
+    StageTimer tm(h, 1);
+    const int nl = launch_fm_raw(b, v, s);
+    if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+    h->launches += nl;
+  }
+  if (h->compute_auc && nrows && d_lab) {
+    DFB_TRY(h->ensure(h->auc_k, nrows * sizeof(float)));
+    DFB_TRY(h->ensure(h->auc_v, nrows * sizeof(float)));
+    DFB_TRY(h->ensure(h->auc_tmp, sort_tmp_bytes(nrows)));
+    StageTimer tm(h, 2);
+    h->launches += launch_auc(d_lab, h->pred.as<float>(), nrows, h->auc_k.as<float>(), h->auc_v.as<float>(),
+                              h->auc_tmp.p, h->auc_tmp.bytes, &h->tab.prog->auc, b.dev_nkeys, s);
+  }
+  if (h->profile) h->prof_steps++;
+  DFB_CUDA(h, cudaGetLastError());
+  return 0;
 }
 
 }  // namespace
@@ -684,7 +740,7 @@ int dfb_destroy(dfb_handle h) {
                     &h->keys, &h->cnt, &h->slot, &h->u_w, &h->u_vrow, &h->flags, &h->pos, &h->lens, &h->cub,
                     &h->gw, &h->gxxp, &h->gV, &h->pred, &h->vals, &h->auc_k, &h->auc_v, &h->a_off, &h->a_idx,
                     &h->a_val, &h->a_lab, &h->a_w, &h->a_wpos, &h->a_vpos, &h->a_pred, &h->a_grad, &h->scal,
-                    &h->hasv, &h->rV, &h->rcg, &h->nvals};
+                    &h->hasv, &h->rV, &h->rcg, &h->nvals, &h->id_ok};
   for (auto* b : bufs) if (b->p) cudaFree(b->p);
   for (auto& s : h->in) {
     DevBuf* ib[] = {&s.off, &s.idx, &s.val, &s.lab, &s.keys, &s.cnt, &s.ids};
@@ -1180,7 +1236,7 @@ int dfbh::stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t n
   else DFB_TRY(h->ensure(in.off, 16));
   DFB_TRY(h2d(h, in.ids, ids, nnz * sizeof(uint64_t), cs));
   if (value) DFB_TRY(h2d(h, in.val, value, nnz * sizeof(float), cs));
-  DFB_TRY(h2d(h, in.lab, label, nrows * sizeof(float), cs));
+  if (label) DFB_TRY(h2d(h, in.lab, label, nrows * sizeof(float), cs));
   DFB_CUDA(h, cudaEventRecord(in.copied, cs));
   return 0;
 }
@@ -1190,14 +1246,13 @@ extern "C" {
 int dfb_prefetch_raw(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
                      const float* label) {
   if (!h) return DFB_ERR_INVALID;
-  DFB_TRY(check_csr(h, nrows, offset));
-  if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
+  DFB_TRY(check_csr(h, nrows, offset));       // (label may be NULL: the batch of a predict step)
   DFB_CUDA(h, cudaSetDevice(h->device));
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
   auto& in = h->in[h->seq & 1];
   DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = ids; in.pre_nrows = nrows; in.pre_nnz = nnz;
+  in.pre_ids = ids; in.pre_lab = label; in.pre_nrows = nrows; in.pre_nnz = nnz;
   return DFB_OK;
 }
 
@@ -1210,8 +1265,7 @@ static int raw_async_impl(dfb_handle h, size_t nrows, const uint64_t* offset, co
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
   auto& in = h->in[h->seq & 1];
-  if (!(in.pre_ids == ids && ids && in.pre_nrows == nrows && in.pre_nnz == nnz))
-    DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
+  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
   in.pre_ids = nullptr;
   DFB_CUDA(h, cudaStreamWaitEvent(h->stream, in.copied, 0));
   int rc = step_raw_dev(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(),
@@ -1221,6 +1275,40 @@ static int raw_async_impl(dfb_handle h, size_t nrows, const uint64_t* offset, co
   h->seq++;
   if (rc != 0) return rc;
   return snapshot_step(h);
+}
+
+int dfb_predict_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
+                          const float* label, float* pred_out) {
+  if (!h) return DFB_ERR_INVALID;
+  if (h->shard)
+    return h->fail(DFB_ERR_INVALID, "this engine holds one shard of a sharded model: predict with dfb_shard_predict_async");
+  DFB_TRY(check_csr(h, nrows, offset));
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
+  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
+  auto& in = h->in[h->seq & 1];
+  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
+  in.pre_ids = nullptr;
+  DFB_CUDA(h, cudaStreamWaitEvent(h->stream, in.copied, 0));
+  int rc = predict_dev(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
+                       label ? in.lab.as<float>() : nullptr, in.copied);
+  // the predictions leave at the end of the step, in stream order (before the next step rewrites h->pred)
+  if (rc == 0 && pred_out && nrows)
+    DFB_CUDA(h, cudaMemcpyAsync(pred_out, h->pred.p, nrows * sizeof(float), cudaMemcpyDeviceToHost, h->stream));
+  DFB_CUDA(h, cudaEventRecord(in.consumed, h->stream));
+  h->seq++;
+  if (rc != 0) return rc;
+  return snapshot_step(h);
+}
+
+int dfb_predict_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
+                        const float* d_value_or_null, const float* d_label_or_null, float* d_pred_out) {
+  if (!h) return DFB_ERR_INVALID;
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  DFB_TRY(predict_dev(h, nrows, nnz, d_offset, d_ids, d_value_or_null, d_label_or_null, nullptr));
+  if (d_pred_out && nrows)
+    DFB_CUDA(h, cudaMemcpyAsync(d_pred_out, h->pred.p, nrows * sizeof(float), cudaMemcpyDeviceToDevice, h->stream));
+  return DFB_OK;
 }
 
 int dfb_train_step_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,

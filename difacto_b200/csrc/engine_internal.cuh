@@ -65,12 +65,17 @@ struct dfb_engine {
   uint64_t or_seq = 0;
   DevBuf a_off, a_idx, a_val, a_lab, a_w, a_wpos, a_vpos, a_pred, a_grad;
   DevBuf scal, hasv, rV, rcg, nvals;
+  DevBuf id_ok;                         // u64: 0 when the raw-id predict step's batch fails its id_bits range check
   // double-buffered inputs of the pipelined step
   struct InSet {
     DevBuf off, idx, val, lab, keys, cnt, ids;
     cudaEvent_t copied = nullptr, consumed = nullptr;
     const void* pre_ids = nullptr;     // host batch already staged by dfb_prefetch_raw (identity check)
+    const void* pre_lab = nullptr;
     size_t pre_nrows = 0, pre_nnz = 0;
+    bool prefetched(const void* ids, const void* lab, size_t nrows, size_t nnz) const {
+      return pre_ids == ids && ids && pre_lab == lab && pre_nrows == nrows && pre_nnz == nnz;
+    }
   } in[2];
   uint64_t seq = 0;
   // per-step Progress snapshots of the pipelined path (pinned ring + completion events)
@@ -154,6 +159,7 @@ int localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
                  const float* d_val, uint64_t max_index, dfb_engine::LocSet& L, cudaStream_t s, bool need_host_U,
                  bool exact_range, size_t* U_out, dfb::DevProgress* drop_prog = nullptr, bool standalone = false);
 int check_csr(dfb_engine* h, size_t nrows, const uint64_t* offset);
+// (label may be NULL: a predict step without labels)
 int stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t nnz, const uint64_t* offset,
               const uint64_t* ids, const float* value, const float* label);
 int collect_one(dfb_engine* h, dfb::DevProgress* acc);

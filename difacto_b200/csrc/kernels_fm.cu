@@ -66,6 +66,23 @@ __device__ __forceinline__ bool batch_dropped(const FmBatch& b, bool raise) {
   return true;
 }
 
+// the raw-id forward: {w, V-row index} of the entry of a raw id, found the way the validation step's find-only
+// k_lookup finds it (the whole 32-byte entry with the first probe, the probe loop only on a collision).  A missing
+// key reads as w = 0 and no V row, what that lookup leaves in the pulled view.
+__device__ __forceinline__ void probe_raw(const FmView& v, unsigned long long id, float& w, int& vr) {
+  const unsigned long long key = raw_key(id);
+  const uint64_t h = hash64(key) & v.tab_mask;
+  const Entry256 e = load_entry(v.tab + h);
+  if (e.key == key) {
+    w = e.w(); vr = e.vrow();
+  } else if (e.key != kEmptyKey) {
+    Table t;
+    t.tab = const_cast<Entry*>(v.tab); t.mask = v.tab_mask;
+    const int s = table_find<false>(t, key, h);
+    if (s >= 0) { w = v.tab[s].w; vr = v.tab[s].vrow; }
+  }
+}
+
 __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, DevProgress* prog) {
   __shared__ float red_s[32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -93,19 +110,26 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 //         the gradient can be reduced per key without atomics (kernels_table.cu: k_bwd_update).
 // MODE 3: owner side of the fused sharded store: partial sums of every worker's rows over this owner's
 //         key segment, stored into the workers' mailboxes (see PartArgs).
+// RAW (MODE 0 only): the nonzeros carry raw feature ids (b.ids); the metadata of each is probed in the table (probe_raw)
+//         instead of being read from a pulled view through a localized index.  Everything after the metadata is
+//         the same code, so the predictions are bit-identical to those of the validation step.
 #ifndef DFB_FM_MINBLOCKS
 #define DFB_FM_MINBLOCKS 4
 #endif
+// The raw-id kernels use the same rule although their metadata chain is longer: prefetching at every K made the K >= 32
+// instantiations spill 130-220 bytes and the flagship predict forward (K = 64) 17 % slower, 0.703 against 0.599 ms
+// (H100 SXM, 700 W).
 #ifndef DFB_FM_PF_MAXK
 #define DFB_FM_PF_MAXK 16       // metadata prefetch (one chunk ahead) for V_dim <= this
 #endif
 #ifndef DFB_FM_MINBLOCKS32
 #define DFB_FM_MINBLOCKS32 DFB_FM_MINBLOCKS     // V_dim = 32 (tuning builds: 3 removes its ~130-byte spills)
 #endif
-template <int K, int MODE, bool HAS_VAL, bool PAD = false>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
 __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MINBLOCKS) k_fm_fast(FmBatch b, FmView v, PartArgs pa) {
   constexpr bool TRAIN = MODE == 1;
   static_assert(!(PAD && TRAIN), "the atomic scatter runs the exact widths only");
+  static_assert(!RAW || MODE == 0, "raw ids are scored, never trained on");
   constexpr int LPR = K / 4;                 // lanes per V row, one float4 each
   constexpr int G = 32 / LPR;                // V rows fetched by one warp-wide load
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;   // independent loads in flight per lane
@@ -147,7 +171,11 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
     auto load_meta = [&](uint64_t c, float& x, float& w, int& vr) {
       const uint64_t j = c + lane;
       x = 0.f; w = 0.f; vr = -1;
-      if (j < o1) {
+      if (RAW && j < o1) {
+        const unsigned long long id = __ldg(reinterpret_cast<const unsigned long long*>(b.ids) + j);
+        x = HAS_VAL ? __ldg(valp + j) : 1.f;
+        probe_raw(v, id, w, vr);
+      } else if (j < o1) {
         const uint32_t u = __ldg(idxp + j);
         x = HAS_VAL ? __ldg(valp + j) : 1.f;
         if (wvp) {
@@ -281,8 +309,9 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
 // ---------------------------------------------------------------------------------------
 constexpr int kLongWarps = 8;
 
-template <int K, int MODE, bool HAS_VAL, bool PAD = false>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
 __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v, int scan_rows) {
+  static_assert(!RAW || MODE == 0, "raw ids are scored, never trained on");
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;
@@ -317,7 +346,11 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
         const uint64_t j = c + lane;
         float x = 0.f, w = 0.f;
         int vr = -1;
-        if (j < o1) {
+        if (RAW && j < o1) {
+          const unsigned long long id = __ldg(reinterpret_cast<const unsigned long long*>(b.ids) + j);
+          x = HAS_VAL ? __ldg(b.value + j) : 1.f;
+          probe_raw(v, id, w, vr);
+        } else if (j < o1) {
           const uint32_t u = __ldg(b.index + j);
           x = HAS_VAL ? __ldg(b.value + j) : 1.f;
           if (v.wv) {
@@ -538,7 +571,8 @@ __global__ void k_grad_finalize_dense(int k, int ks, size_t nkeys, const int* ha
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-template <int K, bool PAD>
+// RAW: the predict-only raw-id kernels (launch_fm_raw), the only ones instantiated with it
+template <int K, bool PAD, bool RAW = false>
 int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const int threads = 256;
   size_t need = (b.nrows + 7) / 8;
@@ -546,7 +580,10 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const bool hv = b.value != nullptr;
   PartArgs pa;
   memset(&pa, 0, sizeof(pa));
-  if (b.train && b.emit) {
+  if constexpr (RAW) {
+    if (hv) k_fm_fast<K, 0, true, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+    else    k_fm_fast<K, 0, false, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+  } else if (b.train && b.emit) {
     if (hv) k_fm_fast<K, 2, true, PAD><<<grid, threads, 0, s>>>(b, v, pa);
     else    k_fm_fast<K, 2, false, PAD><<<grid, threads, 0, s>>>(b, v, pa);
   } else if (b.train) {
@@ -562,7 +599,10 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
     const int lgrid = (int)(b.nrows < (size_t)(num_sms() * 4) ? b.nrows : (size_t)(num_sms() * 4));
     int scan = 1;
     while (scan < kLongWarps * 32 && (size_t)lgrid * scan * 2 <= b.nrows) scan *= 2;
-    if (b.train) {
+    if constexpr (RAW) {
+      if (hv) k_fm_long<K, 0, true, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      else    k_fm_long<K, 0, false, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+    } else if (b.train) {
       if (hv) k_fm_long<K, 2, true, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
       else    k_fm_long<K, 2, false, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
     } else {
@@ -599,6 +639,14 @@ int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& p
     constexpr int K = decltype(kc)::value;
     return V_dim == K ? launch_partial_k<K, false>(V_dim, valued, v, pa, s)
                       : launch_partial_k<K, true>(V_dim, valued, v, pa, s);
+  });
+}
+
+int launch_fm_raw(const FmBatch& b, const FmView& v, cudaStream_t s) {
+  if (b.train || !aligned16(v.vbase) || v.vstride % 4 != 0) return -1;
+  return with_lane_width(b.V_dim, [&](auto kc) {
+    constexpr int K = decltype(kc)::value;
+    return b.V_dim == K ? launch_fast_k<K, false, true>(b, v, s) : launch_fast_k<K, true, true>(b, v, s);
   });
 }
 

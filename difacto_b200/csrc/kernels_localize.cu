@@ -17,13 +17,6 @@ namespace dfb {
 
 namespace {
 
-__device__ __forceinline__ unsigned long long reverse_nibbles(unsigned long long x) {
-  // byte reversal, then swap the two nibbles of every byte  == reversing the 16 nibbles
-  x = ((unsigned long long)__byte_perm((unsigned)(x & 0xffffffffULL), 0, 0x0123) << 32) |
-      (unsigned long long)__byte_perm((unsigned)(x >> 32), 0, 0x0123);
-  return ((x & 0x0F0F0F0F0F0F0F0FULL) << 4) | ((x & 0xF0F0F0F0F0F0F0F0ULL) >> 4);
-}
-
 // HI32: the caller knows that only the upper 32 bits of the reversed keys can be non-zero (ids < 2^32): the sort
 // then runs on 32-bit keys (a third less traffic per radix pass); the OR mask still covers all 64 bits, so a wrong
 // assumption is detected by k_emit like any other range violation.
@@ -268,6 +261,26 @@ __global__ void k_raise_err(DevProgress* prog, int code) { raise_err(prog, code)
 
 int launch_raise_err(DevProgress* prog, int code, cudaStream_t s) {
   k_raise_err<<<1, 1, 0, s>>>(prog, code);
+  return 1;
+}
+
+// the range check of a batch that is scored without the localizer: clears *ok when an id (as Localizer(-1) maps it)
+// is not below 2^nbits, i.e. when the localizer's sort over the same range would have dropped the batch
+__global__ void __launch_bounds__(256) k_id_range(const unsigned long long* __restrict__ ids, size_t n, int nbits,
+                                                  unsigned long long* ok) {
+  unsigned long long acc = 0;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
+    const unsigned long long x = __ldg(ids + i);
+    acc |= x == ~0ULL ? 0ULL : x;
+  }
+  if (__any_sync(0xffffffffu, (acc >> nbits) != 0ULL) && (threadIdx.x & 31) == 0) *ok = 0ULL;
+}
+
+int launch_id_range(const uint64_t* ids, size_t n, int nbits, unsigned long long* ok, cudaStream_t s) {
+  if (n == 0 || nbits >= 64) return 0;
+  const size_t need = (n + 255) / 256;
+  const int grid = (int)(need < (size_t)num_sms() * 8 ? need : (size_t)num_sms() * 8);
+  k_id_range<<<grid, 256, 0, s>>>(reinterpret_cast<const unsigned long long*>(ids), n, nbits, ok);
   return 1;
 }
 

@@ -309,11 +309,12 @@ __global__ void __launch_bounds__(256) k_shard_reduce(ReduceArgs a) {
     float pred = wsum + 0.5f * (s1 - acc2);
     if (!PAD || a.V_dim > 0) pred = pred > 20.f ? 20.f : (pred < -20.f ? -20.f : pred);   // fm_loss.h:77,118
     if (!ok) continue;
-    const float label = __ldg(a.label + row);
+    // (no label: a predict step without labels -- the predictions are stored, the loss stays 0)
+    const float label = a.label ? __ldg(a.label + row) : 0.f;
     const float y = label > 0.f ? 1.f : -1.f;
     if (sub == 0) {
       a.pred[row] = pred;
-      loss_acc += logf(1.f + expf(-y * pred));
+      if (a.label) loss_acc += logf(1.f + expf(-y * pred));
     }
     if (a.train) {
       const float p = -y / (1.f + expf(y * pred));

@@ -57,6 +57,8 @@ struct ShardState {
     const float* d_val = nullptr;
     const float* d_lab = nullptr;
     int push_cnt = 0, is_train = 0;
+    bool predict = false;            // a predict step (dfb_shard_*predict*): no penalty, label optional
+    float* pred_out = nullptr;       // host: this rank's predictions, copied at the end of the step
     cudaEvent_t inputs_ready = nullptr, consumed = nullptr;
     LookupArgs la;
     bool auc = false;
@@ -83,9 +85,11 @@ bool dbg_on() {
     }                                                                                              \
   } while (0)
 
+// predict: the step is a predict step (is_train = push_cnt = 0, label may be NULL); pred_out receives the rows'
+// predictions at the end of the step
 int shard_begin(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                 const float* d_val, const float* d_lab, int push_cnt, int is_train, cudaEvent_t inputs_ready,
-                cudaEvent_t consumed) {
+                cudaEvent_t consumed, bool predict = false, float* pred_out = nullptr) {
   ShardState* shp = h->shard;
   if (!shp) return h->fail(DFB_ERR_INVALID, "dfb_shard_init was not called");
   ShardState& sh = *shp;
@@ -93,12 +97,13 @@ int shard_begin(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, 
   if (sh.cx.open) return h->fail(DFB_ERR_INVALID, "the previous sharded step was not finished (dfb_shard_phase 0..4)");
   if (nrows > sh.Bcap || nnz > sh.Ncap) return h->fail(DFB_ERR_CAPACITY, "batch larger than dfb_shard_init's max_rows / max_nnz");
   if (is_train && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data");   // CHECK(has_aux_), sgd_updater.cc:75
-  if (nrows && !d_lab) return h->fail(DFB_ERR_INVALID, "label is NULL");
+  if (nrows && !d_lab && !predict) return h->fail(DFB_ERR_INVALID, "label is NULL");
   ShardState::Ctx& c = sh.cx;
   c.open = true; c.next_phase = 0;
   c.nrows = nrows; c.nnz = nnz; c.d_off = d_off; c.d_ids = d_ids; c.d_val = d_val; c.d_lab = d_lab;
   c.push_cnt = push_cnt; c.is_train = is_train; c.inputs_ready = inputs_ready; c.consumed = consumed;
-  c.auc = h->compute_auc && nrows;
+  c.predict = predict; c.pred_out = pred_out;
+  c.auc = h->compute_auc && nrows && d_lab;
   return DFB_OK;
 }
 
@@ -145,6 +150,8 @@ int shard_phase(dfb_engine* h, int phase) {
   if (h->profile && h->prof_steps && h->prof_steps % dfb_engine::kProfRing == 0) DFB_TRY(dfbh::prof_drain(h));
   DFB_TRY(h->ensure(sh.rowcnt, (size_t)S * (nrows + 1) * sizeof(int)));
   DFB_TRY(h->ensure(sh.pred[d], (nrows ? nrows : 1) * sizeof(float)));
+  // a dropped batch makes no prediction (k_shard_reduce returns at once): its rows read 0
+  if (c.pred_out && nrows) DFB_CUDA(h, cudaMemsetAsync(sh.pred[d].p, 0, nrows * sizeof(float), W));
   {
     StageTimer tm(h, 5, W);
     // a dropped batch (range, or a segment over its capacity below) is reported into this step's own Progress slot:
@@ -332,7 +339,7 @@ int shard_phase(dfb_engine* h, int phase) {
                                  occ_r, true, p_r, pxv_r, flags + o, 1, &ap, hp.part ? &hp : nullptr, 0, O);
       if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported V_dim for the sharded store");
       h->launches += nl;
-    } else {
+    } else if (!c.predict) {      // (a predict step is collective: every worker's Progress has penalty 0)
       h->launches += launch_penalty(h->prm, sh.src_prog(r), la.w + o, la.vrow + o, h->tab.V, h->tab.rs, 0, Kseg,
                                     &hdr[r]->nkeys, O);
     }
@@ -361,6 +368,8 @@ int shard_phase(dfb_engine* h, int phase) {
   if (h->submitted - h->collected == (uint64_t)dfb_engine::kRing) DFB_TRY(dfbh::collect_one(h, &h->backlog));
   const int rs = (int)(h->submitted % dfb_engine::kRing);
   DFB_CUDA(h, cudaMemcpyAsync(&h->h_ring[rs], sh.stage(d), sizeof(DevProgress), cudaMemcpyDeviceToHost, F));
+  if (c.pred_out && nrows)
+    DFB_CUDA(h, cudaMemcpyAsync(c.pred_out, sh.pred[d].p, nrows * sizeof(float), cudaMemcpyDeviceToHost, F));
   DFB_CUDA(h, cudaEventRecord(h->ring_done[rs], F));
   h->submitted++;
   DFB_CUDA(h, cudaEventRecord(sh.ev_fin[d], F));
@@ -550,8 +559,7 @@ int dfb_shard_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, con
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
   auto& in = h->in[h->seq & 1];
-  if (!(in.pre_ids == ids && ids && in.pre_nrows == nrows && in.pre_nnz == nnz))
-    DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
+  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
   in.pre_ids = nullptr;
   int rc = shard_step(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
                       in.lab.as<float>(), push_cnt, is_train, in.copied, in.consumed);
@@ -582,6 +590,44 @@ int dfb_shard_begin_async(dfb_handle h, size_t nrows, const uint64_t* offset, co
                        in.lab.as<float>(), push_cnt, is_train, in.copied, in.consumed);
   h->seq++;
   return rc;
+}
+
+}  // extern "C"
+
+namespace {
+// the host-buffer predict step: staged through the double-buffered input sets like dfb_shard_begin_async
+int shard_begin_predict(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
+                        const float* label, float* pred_out) {
+  if (!h) return DFB_ERR_INVALID;
+  DFB_TRY(dfbh::check_csr(h, nrows, offset));
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
+  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
+  auto& in = h->in[h->seq & 1];
+  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
+  in.pre_ids = nullptr;
+  int rc = shard_begin(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
+                       label ? in.lab.as<float>() : nullptr, 0, 0, in.copied, in.consumed, true, pred_out);
+  h->seq++;
+  return rc;
+}
+}  // namespace
+
+extern "C" {
+
+int dfb_shard_begin_predict_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
+                                  const float* value, const float* label, float* pred_out) {
+  return shard_begin_predict(h, nrows, offset, ids, value, label, pred_out);
+}
+
+int dfb_shard_predict_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
+                            const float* label, float* pred_out) {
+  DFB_TRY(shard_begin_predict(h, nrows, offset, ids, value, label, pred_out));
+  for (int ph = 0; ph < 5; ++ph) {
+    int rc = shard_phase(h, ph);
+    if (rc != 0) { h->shard->cx.open = false; return rc; }
+  }
+  return DFB_OK;
 }
 
 int dfb_shard_phase(dfb_handle h, int phase) {

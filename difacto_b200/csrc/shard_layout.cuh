@@ -94,7 +94,7 @@ struct ReduceArgs {
   const float2* part_sc[8];
   float* p_dst[8];
   float* pxv_dst[8];
-  const float* label;
+  const float* label;          // nullptr (predict steps only): no loss
   float* pred;
   DevProgress* prog;
 };

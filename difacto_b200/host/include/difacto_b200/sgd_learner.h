@@ -71,8 +71,9 @@ class SGDLearner : public Learner {
   void RunEpochs();
   void RunEpoch(int epoch, int job_type, sgd::Progress* prog);
   void IterateData(const sgd::Job& job, sgd::Progress* prog);
-  /** num_gpus > 1: one epoch over all N * num_jobs_per_epoch file parts, part i handled by worker i % N */
-  void RunEpochSharded(int epoch, int job_type, sgd::Progress* prog);
+  /** num_gpus > 1: one epoch over all N * num_jobs_per_epoch file parts, part i handled by worker i % N.
+   * pred_out (task=predict): predict steps, and the predictions of every row to that file, in file order */
+  void RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, const std::string* pred_out = nullptr);
   void LoadShards();
   /** engine of GPU r (r = 0: the updater's own) */
   const std::shared_ptr<GpuEngine>& ShardEngine(int r) { return r == 0 ? GetUpdater()->engine() : shard_engines_[r - 1]; }

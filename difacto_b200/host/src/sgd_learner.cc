@@ -4,6 +4,7 @@
 
 #include <cstdint>
 #include <cstdio>
+#include <cstring>
 #include <fstream>
 #include <thread>
 
@@ -132,16 +133,48 @@ void SGDLearner::RunScheduler() {
   }
 }
 
+namespace {
+// a pinned host buffer from dfb_host_alloc (asynchronous copies), grown on demand
+class PinnedBuf {
+ public:
+  PinnedBuf() = default;
+  PinnedBuf(const PinnedBuf&) = delete;
+  PinnedBuf& operator=(const PinnedBuf&) = delete;
+  ~PinnedBuf() { if (p_) dfb_host_free(p_); }
+  template <typename T> T* get(size_t n) {
+    const size_t bytes = n * sizeof(T);
+    if (bytes > cap_) {
+      if (p_) dfb_host_free(p_);
+      p_ = nullptr; cap_ = 0;
+      const size_t want = bytes + bytes / 4 + 256;
+      if (dfb_host_alloc(&p_, want) != DFB_OK) throw Error("dfb_host_alloc failed");
+      cap_ = want;
+    }
+    return static_cast<T*>(p_);
+  }
+
+ private:
+  void* p_ = nullptr;
+  size_t cap_ = 0;
+};
+
+void AddProgress(const dfb_progress& pr, sgd::Progress* prog) {
+  prog->loss += pr.loss; prog->penalty += pr.penalty; prog->auc += pr.auc; prog->nrows += pr.nrows;
+}
+
+void WritePreds(FILE* fo, const real_t* pred, size_t n) {
+  for (size_t i = 0; i < n; ++i) fprintf(fo, "%.9g\n", pred[i]);
+}
+}  // namespace
+
 sgd::Progress SGDLearner::Predict() {
   if (param_.model_in.empty()) throw Error("task=predict needs model_in");
   if (param_.num_gpus > 1) {
-    // the model (one file or any number of parts), re-sharded over and scored by N GPUs (loss / AUC only: the rows
-    // of a step are spread over the workers, so there is no single prediction file to write)
-    if (!param_.pred_out.empty()) throw Error("pred_out needs num_gpus=1 (the predictions of a sharded run are spread over the workers)");
+    // the model (one file or any number of parts), re-sharded over and scored by N GPUs
     LoadShards();
     sgd::Progress prog;
     param_.data_val = param_.data_in;
-    RunEpochSharded(0, sgd::Job::kValidation, &prog);
+    RunEpochSharded(0, sgd::Job::kValidation, &prog, param_.pred_out.empty() ? nullptr : &param_.pred_out);
     if (verbose) printf(" - Prediction: %s, rows = %g\n", prog.TextString().c_str(), prog.nrows);
     return prog;
   }
@@ -151,16 +184,38 @@ sgd::Progress SGDLearner::Predict() {
   sgd::Progress prog;
   const auto& eng = GetUpdater()->engine();
   BatchReader reader(param_.data_in, param_.data_format, 0, 1, 65536u);
-  std::vector<real_t> pred;
+  // predict steps, two in flight: chunk t is on the GPU while the reader parses chunk t+1 and the file receives the
+  // predictions of chunk t-1.  Two pinned input sets and two pinned prediction buffers; set t & 1 is refilled only
+  // after step t-2, which used it, has been collected.
+  struct Set { PinnedBuf off, ids, val, lab, pred; size_t nrows = 0; };
+  Set sets[2];
+  uint64_t t = 0;
+  auto collect = [&](uint64_t step) {
+    dfb_progress pr;
+    eng->Check(dfb_wait_step(eng->handle(), &pr), "dfb_predict_raw_async");
+    AddProgress(pr, &prog);
+    Set& s = sets[step & 1];
+    if (fo) WritePreds(fo, s.pred.get<real_t>(s.nrows), s.nrows);
+  };
   while (reader.Next()) {
     const auto blk = reader.Value();
-    pred.assign(blk.size, 0.f);
-    dfb_progress pr;
-    eng->Check(dfb_train_step_raw(eng->handle(), blk.size, reinterpret_cast<const uint64_t*>(blk.offset), blk.index,
-                                  blk.value, blk.label, 0, 0, &pr, pred.data()), "dfb_train_step_raw");
-    prog.loss += pr.loss; prog.penalty += pr.penalty; prog.auc += pr.auc; prog.nrows += pr.nrows;
-    if (fo) for (real_t p : pred) fprintf(fo, "%.9g\n", p);
+    Set& s = sets[t & 1];
+    const size_t n = blk.size, nnz = blk.offset[blk.size];
+    s.nrows = n;
+    uint64_t* off = s.off.get<uint64_t>(n + 1);
+    uint64_t* ids = s.ids.get<uint64_t>(nnz);
+    real_t* lab = s.lab.get<real_t>(n);
+    real_t* val = blk.value ? s.val.get<real_t>(nnz) : nullptr;
+    memcpy(off, blk.offset, (n + 1) * sizeof(uint64_t));
+    memcpy(ids, blk.index, nnz * sizeof(uint64_t));
+    memcpy(lab, blk.label, n * sizeof(real_t));
+    if (val) memcpy(val, blk.value, nnz * sizeof(real_t));
+    eng->Check(dfb_predict_raw_async(eng->handle(), n, off, ids, val, lab, fo ? s.pred.get<real_t>(n) : nullptr),
+               "dfb_predict_raw_async");
+    if (t >= 1) collect(t - 1);
+    ++t;
   }
+  if (t >= 1) collect(t - 1);
   if (fo) fclose(fo);
   if (verbose) printf(" - Prediction: %s, rows = %g\n", prog.TextString().c_str(), prog.nrows);
   return prog;
@@ -217,11 +272,22 @@ void SGDLearner::RunEpoch(int epoch, int job_type, sgd::Progress* prog) {
 // its parts are exhausted) to ONE collective sharded step.  One host thread drives all N engines and interleaves
 // the five enqueue phases of the step (dfb_shard_begin_async + dfb_shard_phase): nothing in a step waits for
 // the host, so the GPUs run concurrently; the readers parse their next batches on helper threads meanwhile.
-void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog) {
+//
+// pred_out: the rows of part i go to a temporary file <pred_out>.part-<i> (host memory stays bounded), which are
+// concatenated in part order into pred_out at the end and removed.
+void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, const std::string* pred_out) {
   const int N = param_.num_gpus;
   const int nparts = N * param_.num_jobs_per_epoch;
   const bool train = job_type == sgd::Job::kTraining;
   const bool push_cnt = train && epoch == 0;      // sgd_learner.cc:201-202
+  const bool predict = pred_out != nullptr;
+  auto tmp_name = [&](int part) { return *pred_out + ".part-" + std::to_string(part); };
+  std::vector<FILE*> part_files(predict ? nparts : 0, nullptr);
+  std::vector<PinnedBuf> pred_bufs(predict ? N : 0);
+  std::vector<int> step_part(N, -1);
+  auto close_parts = [&]() {
+    for (auto& f : part_files) if (f) { fclose(f); f = nullptr; }
+  };
   struct Worker {
     int part = 0;
     std::unique_ptr<BatchReader> reader;
@@ -259,19 +325,23 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog) {
     }
     bool any = false;
     for (int r = 0; r < N; ++r) {
-      if (!w[r].error.empty()) throw Error("worker " + std::to_string(r) + ": " + w[r].error);
+      if (!w[r].error.empty()) { close_parts(); throw Error("worker " + std::to_string(r) + ": " + w[r].error); }
       any = any || w[r].has;
     }
     if (!any) break;
     for (int r = 0; r < N; ++r) {
       const auto& eng = ShardEngine(r);
-      if (w[r].has) {
-        const auto blk = w[r].reader->Value();
-        eng->Check(dfb_shard_begin_async(eng->handle(), blk.size, reinterpret_cast<const uint64_t*>(blk.offset), blk.index,
-                                         blk.value, blk.label, push_cnt ? 1 : 0, train ? 1 : 0), "dfb_shard_begin_async");
+      dmlc::RowBlock<feaid_t> blk;
+      if (w[r].has) blk = w[r].reader->Value();
+      step_part[r] = w[r].has ? w[r].part : -1;
+      const uint64_t* off = blk.size ? reinterpret_cast<const uint64_t*>(blk.offset) : nullptr;
+      if (predict) {       // every rank predicts in the same step (the step is collective)
+        eng->Check(dfb_shard_begin_predict_async(eng->handle(), blk.size, off, blk.index, blk.value, blk.label,
+                                                 pred_bufs[r].get<real_t>(blk.size ? blk.size : 1)),
+                   "dfb_shard_begin_predict_async");
       } else {
-        eng->Check(dfb_shard_begin_async(eng->handle(), 0, nullptr, nullptr, nullptr, nullptr, push_cnt ? 1 : 0, train ? 1 : 0),
-                   "dfb_shard_begin_async");
+        eng->Check(dfb_shard_begin_async(eng->handle(), blk.size, off, blk.index, blk.value, blk.label, push_cnt ? 1 : 0,
+                                         train ? 1 : 0), "dfb_shard_begin_async");
       }
     }
     for (int ph = 0; ph < 5; ++ph)
@@ -280,8 +350,31 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog) {
       dfb_progress pr;
       ShardEngine(r)->Check(dfb_wait_step(ShardEngine(r)->handle(), &pr), "dfb_wait_step");
       prog->loss += pr.loss; prog->penalty += pr.penalty; prog->auc += pr.auc; prog->nrows += pr.nrows;
+      if (predict && step_part[r] >= 0) {
+        FILE*& f = part_files[step_part[r]];
+        if (!f && !(f = fopen(tmp_name(step_part[r]).c_str(), "w"))) {
+          close_parts();
+          throw Error("failed to open " + tmp_name(step_part[r]));
+        }
+        const size_t n = w[r].reader->Value().size;
+        WritePreds(f, pred_bufs[r].get<real_t>(n ? n : 1), n);
+      }
     }
   }
+  if (!predict) return;
+  close_parts();
+  FILE* fo = fopen(pred_out->c_str(), "w");
+  if (!fo) throw Error("failed to open pred_out " + *pred_out);
+  std::vector<char> buf(1 << 20);
+  for (int i = 0; i < nparts; ++i) {
+    FILE* fi = fopen(tmp_name(i).c_str(), "r");
+    if (!fi) continue;        // a part without rows
+    size_t n;
+    while ((n = fread(buf.data(), 1, buf.size(), fi)) > 0) fwrite(buf.data(), 1, n, fo);
+    fclose(fi);
+    std::remove(tmp_name(i).c_str());
+  }
+  fclose(fo);
 }
 
 // SGDLearner::GetPos, sgd_learner.cc:113-127

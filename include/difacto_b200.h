@@ -214,12 +214,34 @@ int dfb_train_step_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset,
                              const float* value_or_null, const float* label, int push_cnt,
                              int is_train);
 /* optional double-buffering hint: start the H2D copy of the batch the NEXT dfb_train_step_raw_async call
- * will be given (same pointers), so that the copy overlaps the step submitted before it */
+ * (or dfb_predict_raw_async / sharded step) will be given (same pointers, label included; it may be NULL for a
+ * predict step), so that the copy overlaps the step submitted before it */
 int dfb_prefetch_raw(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
                      const float* value_or_null, const float* label);
 int dfb_train_step_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset,
                            const uint64_t* d_ids, const float* d_value_or_null, const float* d_label,
                            int push_cnt, int is_train);
+
+/* predict steps on raw ids: the forward pass of a frozen model.  A predict step writes nothing of the model (table,
+ * V rows, AdaGrad state, InitV stream) and runs neither the localizer, the key lookup nor the penalty: for
+ * 0 <= V_dim <= 128 (and force_generic = 0) it is one forward launch whose kernels look each nonzero's id up in the
+ * table themselves; other configurations run the validation step (dfb_train_step_raw with is_train = 0) minus its
+ * penalty.  The predictions are bit-identical to those of that validation step.  Progress: loss and AUC (0 without
+ * labels) and nrows; penalty, new_keys and new_vrows are 0.  id_bits > 0 keeps its meaning: a batch with an id at or
+ * above 2^(4*ceil(id_bits/4)) is dropped (predictions 0, nothing in Progress, DFB_ERR_INVALID once on its read);
+ * with id_bits = 0 every id is scored.
+ *   dfb_predict_raw_async  host buffers, staged through the double-buffered input sets (dfb_prefetch_raw applies);
+ *                          the copy of the nrows predictions into pred_out_or_null is enqueued at the end of the step:
+ *                          pinned memory keeps it asynchronous, and it must stay valid until the step is collected
+ *                          (dfb_wait_step / dfb_read_progress / dfb_sync).  Takes its place in the Progress ring of the
+ *                          other async steps, and sees the updates of the training steps enqueued before it.
+ *   dfb_predict_raw_dev    device buffers, enqueue only (the Progress accumulates as for dfb_train_step_raw_dev);
+ *                          d_pred_out_or_null receives the predictions in stream order.
+ * An engine that is a rank of the sharded store (dfb_shard_init) refuses both: DFB_ERR_INVALID. */
+int dfb_predict_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
+                          const float* value_or_null, const float* label_or_null, float* pred_out_or_null);
+int dfb_predict_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
+                        const float* d_value_or_null, const float* d_label_or_null, float* d_pred_out_or_null);
 
 /* blocks until the OLDEST not yet collected dfb_train_step_async step has finished and
  * returns that step's Progress (each async step snapshots its Progress into a pinned ring,
@@ -395,6 +417,16 @@ int dfb_shard_begin_async(dfb_handle h, size_t nrows, const uint64_t* offset, co
 int dfb_shard_begin_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
                         const float* d_value_or_null, const float* d_label, int push_cnt, int is_train);
 int dfb_shard_phase(dfb_handle h, int phase);
+/* A predict step of the sharded store: the step with is_train = 0 and push_cnt = 0, except that the owners evaluate no
+ * penalty (Progress: loss, AUC, nrows; 0 loss and AUC without labels) and that pred_out_or_null receives this rank's
+ * nrows predictions at the end of the step (pinned memory keeps the copy asynchronous; valid until the step is
+ * collected).  Collective like every step: every rank calls a predict form in the same step.  The predictions equal
+ * those of one engine holding the whole model up to the order of the owners' partial sums.
+ * dfb_shard_begin_predict_async is followed by dfb_shard_phase(0..4), as dfb_shard_begin_async. */
+int dfb_shard_predict_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
+                            const float* value_or_null, const float* label_or_null, float* pred_out_or_null);
+int dfb_shard_begin_predict_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
+                                  const float* value_or_null, const float* label_or_null, float* pred_out_or_null);
 int dfb_shard_info(dfb_handle h, int* rank, int* nranks, size_t* seg_keys, size_t* seg_nnz, uint64_t* steps);
 
 /* the CUDA stream (cudaStream_t) the handle enqueues on, for event interop with torch */
