@@ -318,6 +318,7 @@ size_t localize_sort_tmp_bytes(size_t nnz);
 // hi32: sort on the upper 32 key bits only (the caller knows the lower 32 are zero: ids < 2^32); verified on the device
 // pay / spay: 8 bytes per nnz, the sort payload (and on the 64-bit-key path the row of every nnz); see
 // kernels_localize.cu.  offset must describe the nnz ids as CSR: positions no row covers are not localized.
+// lidx_out may be nullptr when nothing reads the remapped CSR index.
 int launch_localize_keys(const uint64_t* ids, size_t nnz, uint64_t max_index, unsigned long long* rkeys, void* pay,
                          unsigned long long* or_all, const uint64_t* offset, size_t nrows, bool hi32, cudaStream_t s);
 int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_t nnz, int begin_bit,
@@ -341,7 +342,10 @@ int launch_csc_build(const uint32_t* lidx, const void* occ, bool valued, size_t 
 // per key: grad = sum_occ x * pXV[row] - V * XXp, then either FTRL/AdaGrad in place (apply) or
 // complete dense gradient rows out (gw_out, gV_out = sum - V_pulled*XXp; the sharded worker).
 // l2hint: the L2 plan of the single-GPU step (p*XV / p kept, [V|cg] rows streamed); ignored when shard != nullptr.
-int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pull_vrow, size_t n,
+// keys != nullptr (the single-GPU step without a lookup): the kernel finds or inserts every key of keys[n] itself and
+// writes its slot (or -1) into slot[n], what the InitV pass reads.  keys == nullptr (a step that ran k_lookup, and the
+// owner side of the sharded store): the slots and pulled V-row indices of that lookup come in slot / pull_vrow.
+int launch_bwd_update(Table& t, const Params& p, const uint64_t* keys, int* slot, const int* pull_vrow, size_t n,
                       const unsigned long long* dn, const int* col_start, const int* col_end,
                       const void* occ_sorted, bool valued, const float* p_row, const float* pxv, int* flags,
                       int accumulate_penalty, const ShardApply* shard, const HotPart* hot, int l2hint, cudaStream_t s);

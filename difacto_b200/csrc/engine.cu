@@ -213,15 +213,29 @@ int ensure_sorted_ws(dfb_engine* h, size_t nrows, size_t nnz, size_t U, bool val
   return 0;
 }
 
+// the keys a batch of n nonzeros can hold: n, or fewer when ids below 2^id_bits bound them
+size_t key_bound(const dfb_engine* h, size_t n) {
+  return (h->id_bits > 0 && h->id_bits < 40) ? std::min(n, (size_t)1 << h->id_bits) : n;
+}
+
+// true when the pulled view {w, vrow} (8 bytes per key) of that many keys fits in half the L2
+bool view_fits_l2(size_t keys) { return keys * sizeof(int2) <= l2_bytes() / 2; }
+
 // U is the number of keys, or (dU != nullptr) the capacity of the key arrays with the actual count on the device
 // (a batch localized on the GPU never reports its size to the host); d_cnt / cnt_cols: see launch_feacnt.
 // predict: a predict step (dfb_predict_raw_* on widths without the raw-id kernels): no penalty; d_lab may be NULL.
+// d_ids: the batch's raw ids (a sorted training step on the GPU localizer's CSC view, without a feature-count push):
+// no key lookup and no pulled view -- the forward probes the table with each nonzero's id, the update finds or
+// inserts the keys itself -- and d_idx is not read.
 int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint32_t* d_idx,
              const float* d_val, const float* d_lab, const uint64_t* d_keys, size_t U, const float* d_cnt,
              int is_train, const dfb_engine::LocSet* csc = nullptr, const unsigned long long* dU = nullptr,
-             const int* cnt_cols = nullptr, bool predict = false) {
+             const int* cnt_cols = nullptr, bool predict = false, const uint64_t* d_ids = nullptr) {
   const bool csc_ready = csc != nullptr;
   const bool push_cnt = d_cnt != nullptr || cnt_cols != nullptr;
+  const bool probe = d_ids != nullptr;
+  if (probe && !(is_train && h->sorted_path() && csc_ready && !push_cnt))
+    return h->fail(DFB_ERR_INVALID, "the lookup-free step is a sorted training step on the GPU localizer's output");
   if (U > 0x7fffffffULL || nrows > 0x7fffffffULL || nnz > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "batch too large");
   if (is_train && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data");   // CHECK(has_aux_), sgd_updater.cc:75
@@ -236,7 +250,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   int* flags = h->flags.as<int>();
   int* pos = h->pos.as<int>();
   if (h->profile && h->prof_steps && h->prof_steps % dfb_engine::kProfRing == 0) DFB_TRY(prof_drain(h));
-  // Push(kFeaCount) then Pull (sgd_learner.cc:214-217, :177)
+  // Push(kFeaCount) then Pull (sgd_learner.cc:214-217, :177).  The lookup-free step has neither: its stage 0 is empty.
   {
   StageTimer tm(h, 0);
   // a validation / prediction batch must not grow the table: a missing entry reads as w = 0, no V
@@ -246,22 +260,26 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     h->launches += launch_lookup(h->tab, d_keys, U, dU, true, slot, nullptr, nullptr, nullptr, s);
     h->launches += launch_feacnt(h->tab, h->prm, slot, U, dU, d_cnt, cnt_cols, flags, pos, s);
     h->launches += launch_pull_view(h->tab, slot, U, dU, u_w, u_vrow, h->u_wv.as<int2>(), s);
-  } else {
+  } else if (!probe) {
     h->launches += launch_lookup(h->tab, d_keys, U, dU, insert, slot, u_w, u_vrow, h->u_wv.as<int2>(), s);
   }
   }
   FmView v;
   memset(&v, 0, sizeof(v));
-  v.wbase = u_w; v.w_pos = nullptr;
-  v.wv = h->u_wv.as<int2>();
-  v.vbase = h->tab.V; v.v_pos = u_vrow; v.vstride = h->tab.rs; v.dense = 0;
+  v.vbase = h->tab.V; v.vstride = h->tab.rs; v.dense = 0;
   v.l2hint = h->l2_hints;
-  // the pulled view {w,vrow} (8 bytes per key) is read once per nnz: keep it in L2 only when it fits with room to spare
-  // (Criteo-shaped batches: at most 2.6 M keys, 20 MB).  At the flagship shape it can be 52 MB, more than an H100's
-  // whole L2, and each key is read about once, so evict_last would only take room from the p*XV rows of the update.
-  // U is the key count or its bound nnz; ids below 2^id_bits also bound it.
-  const size_t u_bound = (h->id_bits > 0 && h->id_bits < 40) ? std::min(U, (size_t)1 << h->id_bits) : U;
-  v.wv_last = h->l2_hints && u_bound * sizeof(int2) <= l2_bytes() / 2;
+  const size_t u_bound = key_bound(h, U);      // U is the key count or its bound nnz
+  if (probe) {
+    v.tab = h->tab.tab; v.tab_mask = h->tab.mask;
+  } else {
+    v.wbase = u_w; v.w_pos = nullptr;
+    v.wv = h->u_wv.as<int2>();
+    v.v_pos = u_vrow;
+    // the pulled view {w,vrow} (8 bytes per key) is read once per nnz: keep it in L2 only when it fits with room to
+    // spare (Criteo-shaped batches: at most 2.6 M keys, 20 MB).  At the flagship shape it can be 52 MB, more than an
+    // H100's whole L2, and each key is read about once, so evict_last would only take room from the p*XV rows.
+    v.wv_last = h->l2_hints && view_fits_l2(u_bound);
+  }
   // the update's L2 plan (p*XV / p kept, the [V|cg] rows streamed past them) pays when the rows a step touches exceed
   // L2.  When they fit (rcv1- and gisette-shaped batches: at most 65536 keys) the default policy is faster: with the
   // plan the rcv1-shaped update took 0.218 ms instead of 0.201 ms (H100 SXM, 700 W).
@@ -291,6 +309,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   b.V_dim = h->prm.V_dim; b.train = is_train; b.prog = h->tab.prog;
   b.long_nnz = (unsigned)h->long_row_nnz; b.nnz_hint = nnz;
   b.dev_nkeys = dU;      // 0 keys for nnz > 0: the localizer dropped the batch; every kernel below then does nothing
+  b.ids = d_ids;
   if (sorted) {
     b.emit = 1; b.p_out = h->p_row.as<float>(); b.pxv_out = h->pxv.as<float>();
     b.occ_row = csc_ready ? nullptr : h->occ.as<uint32_t>();
@@ -298,7 +317,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   }
   if (nrows) {
     StageTimer tm(h, 1);
-    const int nl = launch_fm(b, v, h->force_generic, s);
+    const int nl = probe ? launch_fm_raw(b, v, s) : launch_fm(b, v, h->force_generic, s);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
     h->launches += nl;
   }
@@ -345,8 +364,10 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     DFB_TRY(dfbh::hot_ws(h, U, nnz, &hws));
     h->launches += launch_hot_prereduce(h->prm.V_dim, U, dU, cs, ce, occs, d_val != nullptr, h->p_row.as<float>(),
                                         h->pxv.as<float>(), h->hot_split, hws, &hp, l2_plan, s);
-    int nl = launch_bwd_update(h->tab, h->prm, slot, u_vrow, U, dU, cs, ce, occs, d_val != nullptr, h->p_row.as<float>(),
-                               h->pxv.as<float>(), flags, 1, nullptr, hp.part ? &hp : nullptr, l2_plan, s);
+    // without a lookup the update finds (or inserts) every key itself and leaves its slot for the InitV pass
+    int nl = launch_bwd_update(h->tab, h->prm, probe ? d_keys : nullptr, slot, u_vrow, U, dU, cs, ce, occs, d_val != nullptr,
+                               h->p_row.as<float>(), h->pxv.as<float>(), flags, 1, nullptr, hp.part ? &hp : nullptr,
+                               l2_plan, s);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "sorted scatter unsupported for this V_dim");
     h->launches += nl;
     if (l2_plan)
@@ -403,7 +424,8 @@ int lowest_bit(unsigned long long or_all) {
 // stays on the device (L.dU()) and *U_out is the capacity nnz.
 int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                        const float* d_val, uint64_t max_index, dfb_engine::LocSet& L, cudaStream_t s,
-                       bool need_host_U, bool exact_range, size_t* U_out, DevProgress* drop_prog, bool standalone) {
+                       bool need_host_U, bool exact_range, size_t* U_out, DevProgress* drop_prog, bool standalone,
+                       bool need_lidx) {
   *U_out = 0;
   if (nnz > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "batch too large");   // localizer.cc:19-20
   if (max_index == 0) return h->fail(DFB_ERR_INVALID, "max_index must be > 0");
@@ -460,7 +482,8 @@ int dfbh::localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* 
     int nl = launch_localize_sort(h->l_rkeys.as<unsigned long long>(), h->l_pay.p, nnz, begin_bit, hi32,
                                   h->l_skeys.as<unsigned long long>(), h->l_spay.p, h->l_tmp.p, h->l_tmp.bytes, d_val,
                                   L.keys.as<uint64_t>(),
-                                  L.col_start.as<int>(), L.col_end.as<int>(), L.lidx.as<uint32_t>(),
+                                  L.col_start.as<int>(), L.col_end.as<int>(),
+                                  need_lidx ? L.lidx.as<uint32_t>() : nullptr,
                                   L.occ_sorted.p, scal, drop_prog, s);
     if (nl < 0) return h->fail(DFB_ERR_CUDA, "radix sort / scan of the GPU localizer failed (temporary storage)");
     h->launches += nl;
@@ -491,11 +514,21 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
   if (inputs_ready) DFB_CUDA(h, cudaStreamWaitEvent(ls, inputs_ready, 0));
   if (L.used) DFB_CUDA(h, cudaStreamWaitEvent(ls, L.consumed, 0));
   const bool dev_count_ok = h->sorted_path(is_train);
+  // a sorted training step without a feature-count push looks no key up (step_dev's d_ids): nothing reads the ranks.
+  // A push_cnt step keeps the lookup: Update(kFeaCount) can start InitV before the Pull, so V rows must exist before
+  // the forward; a validation step's penalty reads the pulled view.  So does a batch whose pulled view fits in L2
+  // (few keys, many nonzeros each: Criteo-, gisette- and rcv1-shaped batches): there the forward reads each nonzero's
+  // metadata from L2, where probing the table costs a chain of round trips per nonzero.  Without the lookup, criteo39
+  // steps took 1.02 instead of 0.95 ms and gisette's 1.09 instead of 0.95 ms (H100 80 GB HBM3, 400 W).
+  // (The key-finding update exists with the L2 plan only, which such a batch has when V_dim > 0 and l2_hints is on.)
+  const bool probe = is_train && !push_cnt && dev_count_ok && !predict && !view_fits_l2(key_bound(h, nnz)) &&
+                     h->l2_hints && h->prm.V_dim > 0;
   size_t U = 0;
   if (h->profile && h->prof_steps && h->prof_steps % dfb_engine::kProfRing == 0) DFB_TRY(prof_drain(h));
   {
     StageTimer tm(h, 5, ls);
-    DFB_TRY(localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, L, ls, !dev_count_ok, exact_range, &U));   // Localizer(-1, ...), sgd_learner.cc:203
+    DFB_TRY(localize_dev(h, nrows, nnz, d_off, d_ids, d_val, ~0ULL, L, ls, !dev_count_ok, exact_range, &U, nullptr,
+                         false, !probe));   // Localizer(-1, ...), sgd_learner.cc:203
   }
   const float* d_cnt = nullptr;
   const int* cnt_cols = nullptr;
@@ -516,8 +549,9 @@ int step_raw_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off,
     DFB_TRY(h->ensure(h->pred, nrows * sizeof(float)));       // what dfb_train_step_raw's pred_out copies
     h->launches += launch_raise_err(h->tab.prog, kErrIdRange, h->stream);
   } else {
-    rc = step_dev(h, nrows, nnz, d_off, L.lidx.as<uint32_t>(), d_val, d_lab, L.keys.as<uint64_t>(), U, d_cnt,
-                  is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols, predict);
+    rc = step_dev(h, nrows, nnz, d_off, probe ? nullptr : L.lidx.as<uint32_t>(), d_val, d_lab, L.keys.as<uint64_t>(),
+                  U, d_cnt, is_train, &L, (dev_count_ok && nnz) ? L.dU() : nullptr, cnt_cols, predict,
+                  probe ? d_ids : nullptr);
   }
   DFB_CUDA(h, cudaEventRecord(L.consumed, h->stream));
   L.used = true;

@@ -154,10 +154,12 @@ int ensure_key_ws(dfb_engine* h, size_t n);
 //   *U_out = the unique-key count when need_host_U, else the capacity (nnz); L.dU() holds the count on the device.
 //   A batch whose ids fall outside the sorted range is dropped: 0 keys (nnz > 0), and kErrIdRange is raised into
 //   drop_prog when given (otherwise the caller reports it).  standalone (dfb_localize): the range is measured,
-//   whatever id_bits or the learned range say, and the learned range is left alone.
+//   whatever id_bits or the learned range say, and the learned range is left alone.  need_lidx = false: L.lidx (the
+//   remapped CSR index) is not written, for a step that reads the raw ids instead.
 int localize_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                  const float* d_val, uint64_t max_index, dfb_engine::LocSet& L, cudaStream_t s, bool need_host_U,
-                 bool exact_range, size_t* U_out, dfb::DevProgress* drop_prog = nullptr, bool standalone = false);
+                 bool exact_range, size_t* U_out, dfb::DevProgress* drop_prog = nullptr, bool standalone = false,
+                 bool need_lidx = true);
 int check_csr(dfb_engine* h, size_t nrows, const uint64_t* offset);
 // (label may be NULL: a predict step without labels)
 int stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t nnz, const uint64_t* offset,

@@ -110,9 +110,10 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 //         the gradient can be reduced per key without atomics (kernels_table.cu: k_bwd_update).
 // MODE 3: owner side of the fused sharded store: partial sums of every worker's rows over this owner's
 //         key segment, stored into the workers' mailboxes (see PartArgs).
-// RAW (MODE 0 only): the nonzeros carry raw feature ids (b.ids); the metadata of each is probed in the table (probe_raw)
-//         instead of being read from a pulled view through a localized index.  Everything after the metadata is
-//         the same code, so the predictions are bit-identical to those of the validation step.
+// RAW (MODE 0 and 2): the nonzeros carry raw feature ids (b.ids); the metadata of each is probed in the table
+//         (probe_raw) instead of being read from a pulled view through a localized index.  Everything after the
+//         metadata is the same code, so the predictions (and p, p*XV) are bit-identical to those of the steps that
+//         look the keys up first.  MODE 2 needs the CSC view of the GPU localizer (b.occ_row == nullptr).
 #ifndef DFB_FM_MINBLOCKS
 #define DFB_FM_MINBLOCKS 4
 #endif
@@ -129,7 +130,7 @@ template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
 __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MINBLOCKS) k_fm_fast(FmBatch b, FmView v, PartArgs pa) {
   constexpr bool TRAIN = MODE == 1;
   static_assert(!(PAD && TRAIN), "the atomic scatter runs the exact widths only");
-  static_assert(!RAW || MODE == 0, "raw ids are scored, never trained on");
+  static_assert(!RAW || MODE == 0 || MODE == 2, "raw ids: predict and emit only");
   constexpr int LPR = K / 4;                 // lanes per V row, one float4 each
   constexpr int G = 32 / LPR;                // V rows fetched by one warp-wide load
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;   // independent loads in flight per lane
@@ -311,7 +312,7 @@ constexpr int kLongWarps = 8;
 
 template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
 __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v, int scan_rows) {
-  static_assert(!RAW || MODE == 0, "raw ids are scored, never trained on");
+  static_assert(!RAW || MODE == 0 || MODE == 2, "raw ids: predict and emit only");
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;
@@ -571,7 +572,7 @@ __global__ void k_grad_finalize_dense(int k, int ks, size_t nkeys, const int* ha
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// RAW: the predict-only raw-id kernels (launch_fm_raw), the only ones instantiated with it
+// RAW: the raw-id kernels (launch_fm_raw): predict (MODE 0) or, in a training step, emit (MODE 2)
 template <int K, bool PAD, bool RAW = false>
 int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const int threads = 256;
@@ -581,8 +582,13 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   PartArgs pa;
   memset(&pa, 0, sizeof(pa));
   if constexpr (RAW) {
-    if (hv) k_fm_fast<K, 0, true, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
-    else    k_fm_fast<K, 0, false, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+    if (b.train) {
+      if (hv) k_fm_fast<K, 2, true, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+      else    k_fm_fast<K, 2, false, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+    } else {
+      if (hv) k_fm_fast<K, 0, true, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+      else    k_fm_fast<K, 0, false, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
+    }
   } else if (b.train && b.emit) {
     if (hv) k_fm_fast<K, 2, true, PAD><<<grid, threads, 0, s>>>(b, v, pa);
     else    k_fm_fast<K, 2, false, PAD><<<grid, threads, 0, s>>>(b, v, pa);
@@ -600,8 +606,13 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
     int scan = 1;
     while (scan < kLongWarps * 32 && (size_t)lgrid * scan * 2 <= b.nrows) scan *= 2;
     if constexpr (RAW) {
-      if (hv) k_fm_long<K, 0, true, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
-      else    k_fm_long<K, 0, false, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      if (b.train) {
+        if (hv) k_fm_long<K, 2, true, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+        else    k_fm_long<K, 2, false, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      } else {
+        if (hv) k_fm_long<K, 0, true, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+        else    k_fm_long<K, 0, false, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      }
     } else if (b.train) {
       if (hv) k_fm_long<K, 2, true, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
       else    k_fm_long<K, 2, false, PAD><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
@@ -643,7 +654,9 @@ int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& p
 }
 
 int launch_fm_raw(const FmBatch& b, const FmView& v, cudaStream_t s) {
-  if (b.train || !aligned16(v.vbase) || v.vstride % 4 != 0) return -1;
+  // training: the emit mode over the CSC view the GPU localizer already wrote
+  if (b.train && (!b.emit || b.occ_row != nullptr || b.occ_rowx != nullptr)) return -1;
+  if (!aligned16(v.vbase) || v.vstride % 4 != 0) return -1;
   return with_lane_width(b.V_dim, [&](auto kc) {
     constexpr int K = decltype(kc)::value;
     return b.V_dim == K ? launch_fast_k<K, false, true>(b, v, s) : launch_fast_k<K, true, true>(b, v, s);

@@ -84,8 +84,9 @@ using EmitTileState = cub::ScanTileState<int>;
 __global__ void k_emit_init(EmitTileState ts, int ntiles) { ts.InitializeStatus(ntiles); }
 
 // Emits unique keys, per-key segment bounds, the remapped CSR index and the per-occurrence payload (row [, x]) in
-// key-then-row order.
-template <typename KT>
+// key-then-row order.  RANKS = false: no remapped index (lidx_out is not written; the step that follows probes the
+// table with the raw ids instead), which saves the random 4-byte scatter of the inverse permutation.
+template <typename KT, bool RANKS>
 __global__ void __launch_bounds__(kEmitThreads)
 k_emit(const KT* __restrict__ skeys, const Payload<KT>* __restrict__ spay, const uint32_t* __restrict__ nnz_row,
        size_t n, const float* __restrict__ value, uint64_t* __restrict__ keys_out, int* __restrict__ col_start,
@@ -149,7 +150,7 @@ k_emit(const KT* __restrict__ skeys, const Payload<KT>* __restrict__ spay, const
     uint32_t row = 0;
     if (sizeof(KT) == 4) row = (uint32_t)((unsigned long long)pay[i] >> 32);
     else if (in) row = nnz_row[p];
-    if (in) lidx_out[p] = (uint32_t)r;
+    if (RANKS && in) lidx_out[p] = (uint32_t)r;
     if (value) occ_rowx[j] = ((unsigned long long)row << 32) | (unsigned long long)__float_as_uint(in ? value[p] : 0.f);
     else occ_row[j] = row;
     if (h) {
@@ -240,18 +241,18 @@ int launch_localize_sort(const unsigned long long* rkeys, const void* pay, size_
     const int bb = begin_bit >= 32 ? begin_bit - 32 : 0;
     if (cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, rk, sk, pv, spv, (int)nnz, bb, 32, s) != cudaSuccess) return -1;
     k_emit_init<<<(ntiles + 255) / 256, 256, 0, s>>>(ts, ntiles);
-    k_emit<uint32_t><<<ntiles, kEmitThreads, 0, s>>>(sk, spv, nullptr, nnz, value, keys_out, col_start, col_end,
-                                                     lidx_out, occ_row, occ_rowx, scal,
-                                                     begin_bit >= 32 ? begin_bit : 32, prog, ts);
+    auto emit = lidx_out ? k_emit<uint32_t, true> : k_emit<uint32_t, false>;
+    emit<<<ntiles, kEmitThreads, 0, s>>>(sk, spv, nullptr, nnz, value, keys_out, col_start, col_end, lidx_out, occ_row,
+                                         occ_rowx, scal, begin_bit >= 32 ? begin_bit : 32, prog, ts);
     passes = (32 - bb + 7) / 8;
   } else {
     const auto* pv = static_cast<const uint32_t*>(pay);
     auto* spv = static_cast<uint32_t*>(spay);
     if (cub::DeviceRadixSort::SortPairs(sort_tmp, sort_bytes, rkeys, skeys, pv, spv, (int)nnz, begin_bit, 64, s) != cudaSuccess) return -1;
     k_emit_init<<<(ntiles + 255) / 256, 256, 0, s>>>(ts, ntiles);
-    k_emit<unsigned long long><<<ntiles, kEmitThreads, 0, s>>>(skeys, spv, pv + nnz, nnz, value, keys_out, col_start,
-                                                               col_end, lidx_out, occ_row, occ_rowx, scal, begin_bit,
-                                                               prog, ts);
+    auto emit = lidx_out ? k_emit<unsigned long long, true> : k_emit<unsigned long long, false>;
+    emit<<<ntiles, kEmitThreads, 0, s>>>(skeys, spv, pv + nnz, nnz, value, keys_out, col_start, col_end, lidx_out,
+                                         occ_row, occ_rowx, scal, begin_bit, prog, ts);
     passes = (64 - begin_bit + 7) / 8;
   }
   return 3 + passes;

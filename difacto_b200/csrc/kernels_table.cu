@@ -663,6 +663,11 @@ __device__ __forceinline__ void load_occ(const void* occ, int o, uint32_t& row, 
 // UNRB row-groups in flight; the first occurrence's p*XV row is fetched together with V|cg.
 // SRC 0: gradient reduced from the occurrence lists (fused step / worker).  SRC 1: gradient read
 // from dense rows gw_in[n], gV_in[n][K] that a worker pushed (owner side of the sharded store).
+// SRC 0 with APPLY (the single-GPU step) and keys != nullptr finds or inserts every key itself: lane i reads keys[i],
+// loads the entry at its hash (the whole 32-byte sector, as k_lookup does) and walks the probe chain only when that is
+// not the key; the slot goes to slot_out[i] for the InitV pass.  The keys of a batch are unique, so one lane inserts
+// each of them.  Otherwise (a step that ran k_lookup; SRC 1 / 2) the slots and pulled V-row indices of the earlier
+// lookup come in slot / pull_vrow.
 // PAD (V_dim < K, single-GPU step and SRC 2 only): lanes at or beyond ks = t.ks touch nothing, the per-row buffers
 // (p*XV, hot-key partials, vsave) have stride ks, and the pad columns [V_dim, ks) of the last float4 are not updated.
 // 3 CTAs/SM (80 registers): at 4 (64 registers) sm_90 spills ~100 bytes per thread and the update stage of the
@@ -673,7 +678,7 @@ __device__ __forceinline__ void load_occ(const void* occ, int o, uint32_t& row, 
 #ifndef DFB_BU_UNRB
 #define DFB_BU_UNRB 2
 #endif
-template <int K, bool HAS_VAL, bool APPLY, int SRC = 0, bool HINT = false, bool PAD = false>
+template <int K, bool HAS_VAL, bool APPLY, int SRC = 0, bool HINT = false, bool PAD = false, bool FIND = false>
 __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, Params p, const int* __restrict__ slot,
                                                     const int* __restrict__ pull_vrow, size_t n_cap,
                                                     const unsigned long long* __restrict__ dn,
@@ -685,7 +690,8 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
                                                     int acc_pen, float* __restrict__ gw_out,
                                                     const float* __restrict__ V_pulled,
                                                     float* __restrict__ gV_out, SegDst seg, ShardApply sa,
-                                                    HotPart hp) {
+                                                    HotPart hp, const unsigned long long* __restrict__ keys,
+                                                    int* __restrict__ slot_out) {
   const unsigned n = (unsigned)dev_count(n_cap, dn);     // < 2^31 (checked by the host): 32-bit index math
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
@@ -693,6 +699,9 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
   constexpr int UNRB = NPASS >= DFB_BU_UNRB ? DFB_BU_UNRB : 1;
   constexpr int kHeavy = 64;     // occurrence-list length above which a key is reduced cooperatively
   static_assert(!PAD || (APPLY && SRC != 1), "padded rows: the table-applying update of the fused paths only");
+  // FIND: the single-GPU step without an earlier lookup, keys in, slots out (its own instantiations, so that the
+  // slot-taking ones stay as they were)
+  static_assert(!FIND || (SRC == 0 && APPLY), "the key-finding update is the single-GPU step's");
   const int lane = threadIdx.x & 31, sub = lane % LPR, grp = lane / LPR;
   const int ks = PAD ? t.ks : K;                  // stride of the per-row buffers
   const bool act = !PAD || sub * 4 < ks;          // this lane's float4 holds V columns
@@ -728,17 +737,23 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
     const unsigned i = base + lane;
     const bool active = i < n;
     int s = -1, vr = -1, o0 = 0, o1 = 0;
+    unsigned long long key = 0;
     if (active) {
-      vr = ld_meta(pull_vrow + i);
+      if (FIND) key = HINT ? ldg_u64_pol(keys + i, pol_once) : __ldg(keys + i);
+      else vr = ld_meta(pull_vrow + i);
       if (SRC != 1) { o0 = ld_meta(col_start + i); o1 = ld_meta(col_end + i); }
-      if (APPLY) s = ld_meta(slot + i);
+      if (APPLY && !FIND) s = ld_meta(slot + i);
     }
     // SRC 2 (owner side of the fused sharded store): this key was already updated in this step by a
     // lower-rank worker's push, so the pull-time V row is the saved copy, not the table row
     const int cf = (SRC == 2 && active && sa.conf != nullptr) ? (int)sa.conf[i] : 0;
     Entry* e = nullptr;
     float4 sc = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (APPLY && s >= 0) {
+    // FIND: the entry sector at the key's hash is loaded here and looked at only after the scalar reduction below, so
+    // that its DRAM latency overlaps the occurrence-list loads instead of stalling the lane in front of them
+    Entry256 en;
+    if (FIND && active && key != kEmptyKey) en = load_entry(t.tab + (hash64(key) & t.mask));
+    if (!FIND && APPLY && s >= 0) {
       e = &t.tab[s];
       sc = *reinterpret_cast<const float4*>(&e->fea_cnt);
     }
@@ -796,6 +811,15 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
     }
     if (!HAS_VAL) xxp = gw;
     if (SRC == 1) xxp = 0.f;                    // pushed rows are complete gradients
+    if (FIND && active) {
+      if (key == kEmptyKey) {
+        raise(t.prog, DFB_ERR_INVALID);         // the empty marker is no key (k_lookup reports it the same way)
+      } else {
+        s = find_insert_entry(t, key, hash64(key) & t.mask, en);
+        if (s >= 0) { vr = en.vrow(); sc = en.scalars(); e = &t.tab[s]; }
+      }
+      slot_out[i] = s;
+    }
     if (APPLY) {
       if (s >= 0) {
         if (vr >= 0) vr = SRC == 1 ? e->vrow : vr;   // SRC 1: pull_vrow is the worker's has_V flag
@@ -810,7 +834,7 @@ __global__ void __launch_bounds__(256, DFB_BU_MINBLOCKS) k_bwd_update(Table t, P
           if (fl) e->vrow = -2;
           flags[i] = fl ? 1 : 0;
         } else {
-          flags[i] = (became_nz && p.V_dim > 0 && e->vrow < 0 && sc.x > (float)p.V_threshold) ? 1 : 0;
+          flags[i] = (became_nz && p.V_dim > 0 && (FIND ? vr : e->vrow) < 0 && sc.x > (float)p.V_threshold) ? 1 : 0;
         }
       } else if (active) {
         flags[i] = 0;
@@ -1294,11 +1318,12 @@ int launch_csc_build(const uint32_t* lidx, const void* occ, bool valued, size_t 
   return 2 + (eb + 7) / 8;   // histogram + one onesweep pass per 8 key bits + bounds
 }
 
-int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pull_vrow, size_t n,
+int launch_bwd_update(Table& t, const Params& p, const uint64_t* keys, int* slot, const int* pull_vrow, size_t n,
                       const unsigned long long* dn, const int* col_start, const int* col_end,
                       const void* occ_sorted, bool valued, const float* p_row, const float* pxv, int* flags,
                       int acc_pen, const ShardApply* shard, const HotPart* hot, int l2hint, cudaStream_t s) {
   if (n == 0) return 0;
+  const unsigned long long* k64 = reinterpret_cast<const unsigned long long*>(keys);
   SegDst noseg;
   memset(&noseg, 0, sizeof(noseg));
   ShardApply sa;
@@ -1307,10 +1332,23 @@ int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pul
   HotPart hp;
   memset(&hp, 0, sizeof(hp));
   if (hot) hp = *hot;
-#define DFB_BU_(K, VAL, SRC, HINT, PAD)                                                                        \
-  k_bwd_update<K, VAL, true, SRC, HINT, PAD><<<grid, 256, 0, s>>>(t, p, slot, pull_vrow, n, dn, col_start, col_end,  \
-                                                             occ_sorted, p_row, pxv, flags, acc_pen, nullptr, nullptr, \
-                                                             nullptr, noseg, sa, hp)
+#define DFB_BU_(K, VAL, SRC, HINT, PAD, FIND)                                                                  \
+  k_bwd_update<K, VAL, true, SRC, HINT, PAD, FIND><<<grid, 256, 0, s>>>(t, p, slot, pull_vrow, n, dn, col_start,     \
+                                                             col_end, occ_sorted, p_row, pxv, flags, acc_pen, nullptr, \
+                                                             nullptr, nullptr, noseg, sa, hp, k64, slot)
+  // the single-GPU step: finding the keys (keys != nullptr; only with the L2 plan, which every batch too large for the
+  // lookup has) or taking the slots of k_lookup
+#define DFB_BU0_(K, PAD)                                                                                       \
+  do {                                                                                                         \
+    if (keys) {                                                                                                \
+      if (!l2hint) return -1;                                                                                  \
+      if (valued) DFB_BU_(K, true, 0, true, PAD, true); else DFB_BU_(K, false, 0, true, PAD, true);            \
+    } else if (l2hint) {                                                                                       \
+      if (valued) DFB_BU_(K, true, 0, true, PAD, false); else DFB_BU_(K, false, 0, true, PAD, false);          \
+    } else {                                                                                                   \
+      if (valued) DFB_BU_(K, true, 0, false, PAD, false); else DFB_BU_(K, false, 0, false, PAD, false);        \
+    }                                                                                                          \
+  } while (0)
   // one short-lived CTA per 256 keys, so that the higher-priority streams working on the NEXT step (localizer;
   // worker / lookup streams of the sharded store) get SM slots as CTAs retire -- a grid-stride grid holds every
   // slot until the kernel ends
@@ -1318,19 +1356,18 @@ int launch_bwd_update(Table& t, const Params& p, const int* slot, const int* pul
   return with_lane_width(p.V_dim, [&](auto kc) {
     constexpr int K = decltype(kc)::value;
     if (p.V_dim == K) {
-      if (shard)       { if (valued) DFB_BU_(K, true, 2, false, false); else DFB_BU_(K, false, 2, false, false); }
-      else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true, false); else DFB_BU_(K, false, 0, true, false); }
-      else             { if (valued) DFB_BU_(K, true, 0, false, false); else DFB_BU_(K, false, 0, false, false); }
+      if (shard) { if (valued) DFB_BU_(K, true, 2, false, false, false); else DFB_BU_(K, false, 2, false, false, false); }
+      else DFB_BU0_(K, false);
     } else {
       if (shard) {
         if (!valued) return -1;         // the owners' wire format is always valued (kernels_shard.cu)
-        DFB_BU_(K, true, 2, false, true);
+        DFB_BU_(K, true, 2, false, true, false);
       }
-      else if (l2hint) { if (valued) DFB_BU_(K, true, 0, true, true); else DFB_BU_(K, false, 0, true, true); }
-      else             { if (valued) DFB_BU_(K, true, 0, false, true); else DFB_BU_(K, false, 0, false, true); }
+      else DFB_BU0_(K, true);
     }
     return 1;
   });
+#undef DFB_BU0_
 #undef DFB_BU_
 }
 
@@ -1387,9 +1424,9 @@ int launch_bwd_dense(const Params& p, DevProgress* prog, int ks, const float* w_
     if (p.V_dim != K) return -1;        // exact widths only
     const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);
     if (valued) k_bwd_update<K, true, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end,
-                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);
+                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp, nullptr, nullptr);
     else k_bwd_update<K, false, false><<<grid, 256, 0, s>>>(t, p, w_alias, hasv, n, nullptr, col_start, col_end,
-                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp);
+                   occ_sorted, p_row, pxv, nullptr, acc_pen, gw_out, V_pulled, gV_out, sd, nosa, nohp, nullptr, nullptr);
     return 1;
   });
 }
@@ -1410,7 +1447,8 @@ int launch_update_pushed(Table& t, const Params& p, const int* slot, const int* 
     if (p.V_dim != K) return -1;        // exact widths only
     const int grid = grid_warps((n + 31) / 32, 8, num_sms() * 8);
     k_bwd_update<K, false, true, 1><<<grid, 256, 0, s>>>(t, p, slot, hasv, n, nullptr, nullptr, nullptr, nullptr, gw,
-                                                          gV, flags, 0, nullptr, nullptr, nullptr, noseg, nosa, nohp);
+                                                          gV, flags, 0, nullptr, nullptr, nullptr, noseg, nosa, nohp,
+                                                          nullptr, nullptr);
     return 1;
   });
 }

@@ -335,7 +335,7 @@ int shard_phase(dfb_engine* h, int phase) {
       h->launches += launch_hot_prereduce(K, Kseg, &hdr[r]->nkeys, cstart, cstart + 1, occ_r, true, p_r, pxv_r,
                                           h->hot_split, hws, &hp, 0, O);
       DFB_DBG(h, "hot-key pre-reduction");
-      int nl = launch_bwd_update(tt, h->prm, la.slot + o, la.vrow + o, Kseg, &hdr[r]->nkeys, cstart, cstart + 1,
+      int nl = launch_bwd_update(tt, h->prm, nullptr, la.slot + o, la.vrow + o, Kseg, &hdr[r]->nkeys, cstart, cstart + 1,
                                  occ_r, true, p_r, pxv_r, flags + o, 1, &ap, hp.part ? &hp : nullptr, 0, O);
       if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported V_dim for the sharded store");
       h->launches += nl;
