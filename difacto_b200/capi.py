@@ -160,7 +160,11 @@ def shard_bounds(sorted_keys, S):
 
 
 class Engine:
-    """One shard of the model on one GPU (wraps a dfb_handle)."""
+    """One shard of the model on one GPU (wraps a dfb_handle).
+
+    The keyword arguments are dfb_create's keys (include/difacto_b200.h).  table_capacity / V_capacity are the initial
+    capacities; with table_capacity_max / V_capacity_max above them the table and the V-row pool grow on demand, and
+    table_stats() reports the current capacities."""
 
     def __init__(self, **kwargs):
         L = lib()

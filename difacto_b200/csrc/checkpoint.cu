@@ -243,6 +243,8 @@ int restore_read(dfb_engine* h, dfb_read_fn fn, void* ctx, uint32_t part, uint32
       wk.have_hdr = true;
       wk.aux = wk.hd.has_aux != 0;
       pos = sizeof(SnapHeader);
+      // room for the whole stream before the first record is inserted (an engine below its maximum grows)
+      DFB_TRY(dfbh::reserve(h, wk.hd.n_keys, wk.hd.n_vrows));
     }
     const size_t fixed = fixed_bytes(wk.aux), rowb = row_bytes(k, wk.aux);
     const size_t start = pos;

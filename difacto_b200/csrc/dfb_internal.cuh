@@ -55,7 +55,7 @@ struct TableState {
 
 struct Table {
   Entry* tab = nullptr;
-  uint64_t cap = 0, mask = 0, max_keys = 0;
+  uint64_t cap = 0, mask = 0, max_keys = 0;   // slots (power of 2, >= 2 max_keys), cap - 1, keys it may hold
   float* V = nullptr;
   float* Vcg = nullptr;
   uint64_t vcap = 0;
@@ -235,6 +235,8 @@ int launch_grad_finalize_dense(int V_dim, int ks, size_t nkeys, const int* hasv,
 
 // ---- launchers (kernels_table.cu) ----
 int launch_table_init(Table& t, unsigned seed, cudaStream_t s);
+// empties new_t (new_t.cap >= old_t.cap slots) and re-inserts every entry of old_t into it, bytes unchanged
+int launch_table_rehash(const Table& old_t, const Table& new_t, cudaStream_t s);
 // find (or insert) keys; slot_out[i] = hash position or -1.  When pull outputs are non-null also
 // emits w and vrow of each entry.
 // n is a host count, or (dn != nullptr) the capacity with the actual count read from the device

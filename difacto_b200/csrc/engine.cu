@@ -240,6 +240,8 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
     return h->fail(DFB_ERR_INVALID, "batch too large");
   if (is_train && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data");   // CHECK(has_aux_), sgd_updater.cc:75
   const bool sorted = is_train && h->sorted_path();
+  // a training or feature-count step inserts at most U keys (U: the key count or its bound nnz), each with a V row
+  if (is_train || push_cnt) DFB_TRY(dfbh::reserve(h, U, U));
   const int ks = h->tab.ks;
   cudaStream_t s = h->stream;
   DFB_TRY(ensure_key_ws(h, U));
@@ -640,7 +642,7 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   Params& p = h->prm;
   p.l1 = 1.f; p.l2 = 0.f; p.V_l2 = .01f; p.lr = .01f; p.lr_beta = 1.f; p.V_lr = .01f; p.V_lr_beta = 1.f;
   p.V_init_scale = .01f; p.V_threshold = 10; p.V_dim = -1; p.seed = 0;
-  long long table_capacity = 1 << 20, v_capacity = -1;
+  long long table_capacity = 1 << 20, v_capacity = -1, table_capacity_max = -1, v_capacity_max = -1;
   struct FR { const char* name; float* dst; float lo, hi; };
   FR fr[] = {{"l1", &p.l1, 0, 1e10f}, {"l2", &p.l2, 0, 1e10f}, {"V_l2", &p.V_l2, 0, 1e10f},
              {"lr", &p.lr, 0, 10}, {"lr_beta", &p.lr_beta, 0, 1e10f}, {"V_lr", &p.V_lr, 0, 1e10f},
@@ -675,6 +677,8 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else if (k == "device") { if (!need_int(0, 1023)) { delete h; return DFB_ERR_PARAM; } h->device = (int)x; }
     else if (k == "table_capacity") { if (!need_int(1, 1LL << 30)) { delete h; return DFB_ERR_PARAM; } table_capacity = x; }
     else if (k == "V_capacity") { if (!need_int(0, 1LL << 30)) { delete h; return DFB_ERR_PARAM; } v_capacity = x; }
+    else if (k == "table_capacity_max") { if (!need_int(1, 1LL << 30)) { delete h; return DFB_ERR_PARAM; } table_capacity_max = x; }
+    else if (k == "V_capacity_max") { if (!need_int(0, 1LL << 30)) { delete h; return DFB_ERR_PARAM; } v_capacity_max = x; }
     else if (k == "compute_auc") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->compute_auc = (int)x; }
     else if (k == "force_generic") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->force_generic = (int)x; }
     else if (k == "overlap_auc") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->overlap_auc = (int)x; }
@@ -691,8 +695,16 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else h->unknown.push_back(std::make_pair(k, v));
   }
   if (p.V_dim < 0) return bad("Required parameter V_dim of int is not presented");   // sgd_param.h:104
+  // the initial capacities and the maxima they may grow to (equal by default: nothing grows)
+  if (table_capacity_max < 0) table_capacity_max = table_capacity;
+  if (table_capacity_max < table_capacity) return bad("table_capacity_max must be >= table_capacity");
+  if (v_capacity_max < 0) v_capacity_max = v_capacity >= 0 ? v_capacity : table_capacity_max;
   if (v_capacity < 0) v_capacity = table_capacity;
-  if (p.V_dim == 0) v_capacity = 0;
+  if (v_capacity_max < v_capacity) return bad("V_capacity_max must be >= V_capacity");
+  if (p.V_dim == 0) v_capacity = v_capacity_max = 0;
+  h->grow.tab_max = (uint64_t)table_capacity_max;
+  h->grow.v_max = (uint64_t)v_capacity_max;
+  h->grow.on = table_capacity_max > table_capacity || v_capacity_max > v_capacity;
 
   cudaError_t e;
   auto cfail = [&](const char* what) {
@@ -729,12 +741,12 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   t.mask = t.cap - 1;
   t.ks = (p.V_dim + 3) / 4 * 4;
   t.vcap = (uint64_t)v_capacity;
-  if ((e = cudaMalloc(&t.tab, t.cap * sizeof(Entry))) != cudaSuccess) return cfail("cudaMalloc(table)");
   t.rs = 2 * t.ks;
-  if (t.vcap && t.ks) {
-    size_t vb = (size_t)t.vcap * t.rs * sizeof(float);
-    if ((e = cudaMalloc(&t.V, vb)) != cudaSuccess) return cfail("cudaMalloc(V rows)");
-    t.Vcg = t.V + t.ks;
+  if (const int rc = dfbh::capacity_create(h)) {
+    g_create_error = h->err;
+    cudaGetLastError();
+    dfb_destroy(h);
+    return rc;
   }
   if ((e = cudaMalloc(&t.state, sizeof(TableState))) != cudaSuccess) return cfail("cudaMalloc(state)");
   if ((e = cudaMalloc(&t.prog, 2 * sizeof(DevProgress))) != cudaSuccess) return cfail("cudaMalloc(prog)");
@@ -782,8 +794,7 @@ int dfb_destroy(dfb_handle h) {
     if (s.copied) cudaEventDestroy(s.copied);
     if (s.consumed) cudaEventDestroy(s.consumed);
   }
-  if (h->tab.tab) cudaFree(h->tab.tab);
-  if (h->tab.V) cudaFree(h->tab.V);
+  dfbh::capacity_destroy(h);
   if (h->tab.state) cudaFree(h->tab.state);
   if (h->tab.prog) cudaFree(h->tab.prog);
   if (h->h_prog) cudaFreeHost(h->h_prog);
@@ -858,6 +869,7 @@ int dfb_push_feacnt(dfb_handle h, const uint64_t* keys, size_t n, const float* c
   DFB_TRY(h2d(h, h->keys, keys, n * sizeof(uint64_t), s));
   DFB_TRY(h2d(h, h->cnt, cnt, n * sizeof(float), s));
   DFB_TRY(ensure_key_ws(h, n));
+  DFB_TRY(dfbh::reserve(h, n, n));
   h->launches += launch_lookup(h->tab, h->keys.as<uint64_t>(), n, nullptr, true, h->slot.as<int>(), nullptr, nullptr, nullptr, s);
   h->launches += launch_feacnt(h->tab, h->prm, h->slot.as<int>(), n, nullptr, h->cnt.as<float>(), nullptr,
                                h->flags.as<int>(), h->pos.as<int>(), s);
@@ -877,6 +889,7 @@ int dfb_pull(dfb_handle h, const uint64_t* keys, size_t n, float* vals_out, size
   if (n == 0) return DFB_OK;
   DFB_TRY(h2d(h, h->keys, keys, n * sizeof(uint64_t), s));
   DFB_TRY(ensure_key_ws(h, n));
+  DFB_TRY(dfbh::reserve(h, n, 0));     // model_[key] inserts; a pull allocates no V row
   if (k == 0) {
     if (vals_cap < n) return h->fail(DFB_ERR_INVALID, "vals_out too small");
     h->launches += launch_lookup(h->tab, h->keys.as<uint64_t>(), n, nullptr, true, h->slot.as<int>(), h->u_w.as<float>(),
@@ -937,6 +950,7 @@ int dfb_push_grad(dfb_handle h, const uint64_t* keys, size_t n, const float* gra
     d_lens = h->lens.as<int>();
     h->launches += launch_lens_scan(d_lens, n, h->pos.as<int>(), h->cub.p, h->cub.bytes, s);
   }
+  DFB_TRY(dfbh::reserve(h, n, n));
   h->launches += launch_lookup(h->tab, h->keys.as<uint64_t>(), n, nullptr, true, h->slot.as<int>(), nullptr, nullptr, nullptr, s);
   h->launches += launch_update_ragged(h->tab, h->prm, h->slot.as<int>(), n, h->vals.as<float>(), d_lens,
                                       h->pos.as<int>(), h->flags.as<int>(), s);
@@ -1429,6 +1443,7 @@ int dfb_dev_feacnt(dfb_handle h, const uint64_t* d_keys, size_t n, const float* 
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));
+  DFB_TRY(dfbh::reserve(h, n, n));
   cudaStream_t s = h->stream;
   h->launches += launch_lookup(h->tab, d_keys, n, nullptr, true, h->slot.as<int>(), nullptr, nullptr, nullptr, s);
   h->launches += launch_feacnt(h->tab, h->prm, h->slot.as<int>(), n, nullptr, d_cnt, nullptr, h->flags.as<int>(),
@@ -1443,6 +1458,7 @@ static int dev_pull_rows_impl(dfb_handle h, const uint64_t* d_keys, size_t n, fl
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));
+  DFB_TRY(dfbh::reserve(h, n, 0));
   cudaStream_t s = h->stream;
   h->launches += launch_lookup(h->tab, d_keys, n, nullptr, true, h->slot.as<int>(), nullptr, nullptr, nullptr, s);
   h->launches += launch_gather_rows(h->tab, h->slot.as<int>(), n, d_w_out, d_hasv_out, d_hasv_out2,
@@ -1613,6 +1629,7 @@ int dfb_dev_push_rows(dfb_handle h, const uint64_t* d_keys, size_t n, const floa
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));
+  DFB_TRY(dfbh::reserve(h, n, n));
   cudaStream_t s = h->stream;
   h->launches += launch_lookup(h->tab, d_keys, n, nullptr, true, h->slot.as<int>(), nullptr, nullptr, nullptr, s);
   int nl = h->force_generic ? -1 : launch_update_pushed(h->tab, h->prm, h->slot.as<int>(), d_hasv, n, d_gw, d_gV,

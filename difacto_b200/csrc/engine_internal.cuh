@@ -100,6 +100,25 @@ struct dfb_engine {
   unsigned long long* h_nvals = nullptr;  // pinned
   ShardState* shard = nullptr;          // the NVLink-sharded store this engine is a rank of (shard.cu)
 
+  // capacity growth up to table_capacity_max / V_capacity_max (growth.cu)
+  struct Growth {
+    uint64_t tab_max = 0, v_max = 0;
+    bool on = false;                    // a maximum lies above its initial capacity
+    cudaMemPool_t pool = nullptr;       // the table's stream-ordered allocations (release threshold 0)
+    // the V-row pool: address space reserved for v_max rows, physical memory mapped at its start
+    unsigned long long vbase = 0;
+    size_t vreserved = 0, vmapped = 0, gran = 0;
+    std::vector<std::pair<unsigned long long, size_t>> vchunks;   // {allocation handle, bytes}, in address order
+    // the last table counts the host knows, and the insertion bounds enqueued since: each inserting call enqueues a
+    // copy of {n_keys, n_vrows} as they are before it into a pinned ring, read once its event has completed
+    static constexpr int kRing = 8;
+    unsigned long long* h_st = nullptr;             // pinned [kRing][2]
+    cudaEvent_t ev[kRing] = {};
+    uint64_t at_k[kRing] = {}, at_v[kRing] = {};    // the bound totals when the copy was enqueued
+    uint64_t head = 0, seq = 0;                     // ring entries [head, seq) are in flight
+    uint64_t known_k = 0, known_v = 0, known_at_k = 0, known_at_v = 0, total_k = 0, total_v = 0;
+  } grow;
+
   // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (0 <= V_dim <= 128) and,
   // when it trains, the atomic-free sorted gradient reduction
   bool sorted_path(bool is_train = true) const {
@@ -165,6 +184,15 @@ int check_csr(dfb_engine* h, size_t nrows, const uint64_t* offset);
 int stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t nnz, const uint64_t* offset,
               const uint64_t* ids, const float* value, const float* label);
 int collect_one(dfb_engine* h, dfb::DevProgress* acc);
+// growth.cu: the table (h->tab.cap slots) and the V-row pool (h->tab.vcap rows mapped, grow.v_max reserved) at create,
+// and their release
+int capacity_create(dfb_engine* h);
+void capacity_destroy(dfb_engine* h);
+// before a call that can insert up to new_keys keys and new_vrows V rows (enqueued next on h->stream): grows the
+// table and the pool when the known counts plus every bound enqueued since could exceed their capacities.  Never
+// waits for the device, and a failed allocation keeps the current table and pool (a step that really overflows them
+// reports DFB_ERR_CAPACITY).  Does nothing on an engine that cannot grow.
+int reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows);
 void shard_destroy(dfb_engine* h);      // shard.cu
 int shard_sync(dfb_engine* h);          // shard.cu: drain the shard's streams
 }  // namespace dfbh

@@ -555,6 +555,38 @@ __global__ void k_set_state(TableState* st, unsigned long long n_keys, unsigned 
   st->n_keys = n_keys; st->n_vrows = n_vrows; st->seed = seed;
 }
 
+// table growth, two launches of one kernel: phase 0 writes the empty entry into every slot of the new table, phase 1
+// re-inserts every occupied entry of the old one -- all 32 bytes as they are -- with table_find's hash and linear
+// probing.  The keys are unique, so a claimed slot is always an empty one.  TableState is not touched.
+__global__ void __launch_bounds__(256) k_table_rehash(const Entry* __restrict__ old_tab, uint64_t old_cap, Entry* nw,
+                                                      uint64_t nw_mask, int phase) {
+  const size_t i0 = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  ulonglong2* out = reinterpret_cast<ulonglong2*>(nw);
+  if (phase == 0) {
+    for (size_t i = i0; i <= nw_mask; i += stride) {
+      out[2 * i] = make_ulonglong2(kEmptyKey, 0x00000000ffffffffULL);    // {key, vrow -1 | pad 0}
+      out[2 * i + 1] = make_ulonglong2(0ULL, 0ULL);                      // fea_cnt, w, sqrt_g, z
+    }
+    return;
+  }
+  const ulonglong2* in = reinterpret_cast<const ulonglong2*>(old_tab);
+  for (size_t i = i0; i < old_cap; i += stride) {
+    const ulonglong2 a = in[2 * i];
+    if (a.x == kEmptyKey) continue;
+    const ulonglong2 b = in[2 * i + 1];
+    uint64_t h = hash64(a.x) & nw_mask;
+    for (uint64_t probe = 0; probe <= nw_mask; ++probe) {
+      if (atomicCAS(&nw[h].key, kEmptyKey, a.x) == kEmptyKey) {
+        out[2 * h] = a;
+        out[2 * h + 1] = b;
+        break;
+      }
+      h = (h + 1) & nw_mask;
+    }
+  }
+}
+
 // Loss::Evaluate, loss.h:57-66
 __global__ void k_evaluate(const float* __restrict__ label, const float* __restrict__ pred, size_t n, double* out) {
   __shared__ float red_s[32];
@@ -1161,6 +1193,12 @@ size_t l2_bytes() {
 int launch_table_init(Table& t, unsigned seed, cudaStream_t s) {
   k_table_init<<<num_sms() * 8, 256, 0, s>>>(t.tab, t.cap, t.state, t.prog, seed);
   return 1;
+}
+
+int launch_table_rehash(const Table& old_t, const Table& new_t, cudaStream_t s) {
+  k_table_rehash<<<num_sms() * 8, 256, 0, s>>>(old_t.tab, old_t.cap, new_t.tab, new_t.mask, 0);
+  k_table_rehash<<<num_sms() * 8, 256, 0, s>>>(old_t.tab, old_t.cap, new_t.tab, new_t.mask, 1);
+  return 2;
 }
 
 int launch_lookup(Table& t, const uint64_t* keys, size_t n, const unsigned long long* dn, bool insert,

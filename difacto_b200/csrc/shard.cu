@@ -438,6 +438,10 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   if (!h->sorted_path())
     return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in 0..128, scatter=sorted and no force_generic "
                                     "(other configurations: the all_to_all ShardedStore)");
+  // an owner's per-step insertion bound is only known on the host as S x seg_keys: far too much headroom to reserve
+  if (h->grow.on)
+    return h->fail(DFB_ERR_INVALID, "the fused sharded store does not grow its shards: create the engine with "
+                                    "table_capacity_max = table_capacity and V_capacity_max = V_capacity");
   DFB_CUDA(h, cudaSetDevice(h->device));
   ShardState* sh = new ShardState();
   h->shard = sh;

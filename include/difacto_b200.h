@@ -66,8 +66,18 @@ typedef struct {
  *   l1 l2 V_l2 lr lr_beta V_lr V_lr_beta V_init_scale V_dim V_threshold seed
  * plus engine-only keys (unknown to the reference, ignored by it with a warning):
  *   device (0)            CUDA device ordinal
- *   table_capacity (1<<20) max number of distinct keys this shard can hold
- *   V_capacity (=table_capacity) max number of keys with an allocated V row
+ *   table_capacity (1<<20) number of distinct keys this shard can hold at first
+ *   V_capacity (=table_capacity) number of keys with an allocated V row at first
+ *   table_capacity_max (=table_capacity)  the key capacity may grow to this, in [table_capacity, 2^30]
+ *   V_capacity_max (=V_capacity when given, else table_capacity_max)  the V-row capacity may grow to this
+ *                         Before every call that can insert keys (training and feature-count steps, dfb_pull,
+ *                         dfb_push_*, dfb_dev_feacnt / _pull_rows* / _push_rows, restore) the engine grows the table
+ *                         and the V-row pool when the keys it knows of plus an upper bound of that call's insertions
+ *                         (nnz of a raw batch, nkeys, n, a snapshot's counts) could exceed them, up to the maxima,
+ *                         without waiting for the device.  Capacities stay below about twice the keys plus the bounds
+ *                         of the steps in flight.  A growth that cannot get memory keeps the current capacities; a
+ *                         call reports DFB_ERR_CAPACITY exactly when it overflows them.  With both maxima at their
+ *                         defaults nothing grows.  The fused sharded store refuses an engine that can grow.
  *   compute_auc (1)       evaluate AUC on device each step (sgd_learner.cc:150-153)
  *   scatter (sorted)      sorted = gradient reduced per key through a stable radix-sorted CSC view of
  *                         the batch, fused with the FTRL/AdaGrad step (no atomics, bit-reproducible,
@@ -106,7 +116,7 @@ int dfb_num_unknown_kwargs(dfb_handle h);
 int dfb_unknown_kwarg(dfb_handle h, int i, const char** key, const char** val);
 /* number of kernels this handle has launched so far (bench.py's gpu_launches) */
 uint64_t dfb_launch_count(dfb_handle h);
-/* number of keys / V rows currently stored */
+/* number of keys / V rows currently stored, and the current (grown) key and V-row capacities */
 int dfb_table_stats(dfb_handle h, uint64_t* n_keys, uint64_t* n_vrows, uint64_t* capacity,
                     uint64_t* v_capacity);
 

@@ -37,7 +37,8 @@ class GpuSGDUpdater : public SGDUpdater {
       {"seed", std::to_string(p.seed)}};
     KWArgs rest;
     for (const auto& a : remain) {
-      if (a.first == "device" || a.first == "table_capacity" || a.first == "V_capacity" || a.first == "scatter")
+      if (a.first == "device" || a.first == "table_capacity" || a.first == "V_capacity" ||
+          a.first == "table_capacity_max" || a.first == "V_capacity_max" || a.first == "scatter")
         kv.push_back(a);
       else
         rest.push_back(a);
