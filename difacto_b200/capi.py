@@ -35,7 +35,8 @@ EXPORTS = [
     "dfb_peer_alloc", "dfb_peer_open", "dfb_peer_close", "dfb_peer_free", "dfb_dev_pull_rows_peer",
     "dfb_dev_fm_step_peer", "dfb_localize", "dfb_train_step_raw", "dfb_train_step_raw_async",
     "dfb_train_step_raw_dev", "dfb_prefetch_raw", "dfb_snapshot_size", "dfb_snapshot", "dfb_restore",
-    "dfb_snapshot_write", "dfb_restore_read",
+    "dfb_snapshot_write", "dfb_restore_read", "dfb_snapshot_begin", "dfb_frozen_write", "dfb_frozen_error",
+    "dfb_frozen_release", "dfb_id_range_get", "dfb_id_range_set",
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
     "dfb_predict_raw_async", "dfb_predict_raw_dev", "dfb_shard_predict_async", "dfb_shard_begin_predict_async",
@@ -110,6 +111,13 @@ def lib():
         L.dfb_snapshot_write.argtypes = [vp, C.c_int, sz, WRITE_FN, vp]
         L.dfb_restore_read.argtypes = [vp, READ_FN, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, sz,
                                        C.POINTER(C.c_int)]
+        L.dfb_snapshot_begin.argtypes = [vp, C.c_int, C.POINTER(vp)]
+        L.dfb_frozen_write.argtypes = [vp, sz, WRITE_FN, vp]
+        L.dfb_frozen_error.restype = C.c_char_p
+        L.dfb_frozen_error.argtypes = [vp]
+        L.dfb_frozen_release.argtypes = [vp]
+        L.dfb_id_range_get.argtypes = [vp, C.POINTER(C.c_int)]
+        L.dfb_id_range_set.argtypes = [vp, C.c_int]
         L.dfb_shard_init.argtypes = [vp, C.c_int, C.c_int, sz, sz, sz, sz, C.POINTER(sz)]
         L.dfb_shard_export.argtypes = [vp, C.POINTER(vp), vp]
         L.dfb_shard_connect.argtypes = [vp, vp]
@@ -144,6 +152,43 @@ def _p(a):
 
 def _arr(a, dt):
     return None if a is None else np.ascontiguousarray(a, dtype=dt)
+
+
+def _write_cb(fileobj, failed):
+    def write(_ctx, buf, n):
+        try:
+            fileobj.write(C.string_at(buf, n))
+            return 0
+        except Exception as e:     # reported after the C call returns
+            failed.append(e)
+            return 1
+    return WRITE_FN(write)
+
+
+class Frozen:
+    """a snapshot frozen on the device by Engine.snapshot_begin (wraps a dfb_frozen).  write_to may run on another
+    thread while the engine trains; release frees the copy (closing the engine frees one not released, after which
+    write_to refuses and release does nothing)."""
+
+    def __init__(self, engine, f):
+        self.engine, self.f, self.L = engine, f, engine.L
+
+    def write_to(self, fileobj, chunk_bytes=0):
+        if not self.f:
+            raise DfbError(DFB_ERR_INVALID, "the frozen snapshot was released")
+        failed = []
+        cb = _write_cb(fileobj, failed)
+        rc = self.L.dfb_frozen_write(self.f, int(chunk_bytes), cb, None)
+        if rc != 0:
+            err = DfbError(rc, self.L.dfb_frozen_error(self.f).decode())
+            if failed:
+                raise err from failed[0]
+            raise err
+
+    def release(self):
+        if self.f:
+            self.L.dfb_frozen_release(self.f)
+            self.f = None
 
 
 def key_owner(key, S):
@@ -183,6 +228,8 @@ class Engine:
 
     def close(self):
         if getattr(self, "h", None):
+            for f in getattr(self, "_frozen", []):
+                f.f = None           # dfb_destroy releases a frozen snapshot left behind
             self.L.dfb_destroy(self.h)
             self.h = None
 
@@ -418,6 +465,22 @@ class Engine:
         if failed:
             raise DfbError(rc, self.L.dfb_last_error(self.h).decode()) from failed[0]
         self._ck(rc)
+
+    def snapshot_begin(self, save_aux=True):
+        """freeze the model on the device (dfb_snapshot_begin); the engine may train while the copy is written"""
+        f = C.c_void_p()
+        self._ck(self.L.dfb_snapshot_begin(self.h, int(save_aux), C.byref(f)))
+        self._frozen = [x for x in getattr(self, "_frozen", []) if x.f] + [Frozen(self, f)]
+        return self._frozen[-1]
+
+    def id_range(self):
+        """the id range learned so far, as a bit count (0: none yet)"""
+        b = C.c_int()
+        self._ck(self.L.dfb_id_range_get(self.h, C.byref(b)))
+        return b.value
+
+    def set_id_range(self, bits):
+        self._ck(self.L.dfb_id_range_set(self.h, int(bits)))
 
     def restore_from(self, fileobj, part=0, nparts=1, shard=0, nshards=1, chunk_bytes=0):
         """restore (merge) one snapshot stream read from fileobj.read (dfb_restore_read); returns has_aux"""

@@ -35,35 +35,78 @@ constexpr size_t kMaxChunk = size_t(1) << 30;      // record offsets within a ch
 size_t fixed_bytes(bool aux) { return 8 + 4 + 4 + (aux ? 8 : 0) + 4; }
 size_t row_bytes(int k, bool aux) { return (size_t)k * 4 * (aux ? 2 : 1); }
 
-// everything a streamed checkpoint allocates, released on every path out of the call (after the stream drained)
+// where a routine reports its errors: the handle's message, or a frozen copy's own (dfb_frozen_write runs beside
+// the handle's owning thread and must not touch the handle)
+struct ErrSink {
+  std::string* err;
+  int fail(int code, const std::string& msg) { *err = msg; return code; }
+  int cuda_fail(cudaError_t e, const char* what) {
+    *err = std::string(what) + ": " + cudaGetErrorString(e);
+    return DFB_ERR_CUDA;
+  }
+};
+
+// everything a streamed checkpoint allocates, released on every path out of the call (after the stream drained).
+// Device memory is stream-ordered on s, so a writer beside training steps never synchronises the device.
 struct Scratch {
-  dfb_engine* h;
+  ErrSink* es;
+  cudaStream_t s;
   std::vector<void*> dev, host;
   std::vector<cudaEvent_t> ev;
-  explicit Scratch(dfb_engine* h_) : h(h_) {}
+  Scratch(ErrSink* es_, cudaStream_t s_) : es(es_), s(s_) {}
   ~Scratch() {
-    cudaStreamSynchronize(h->stream);
-    for (void* p : dev) cudaFree(p);
+    for (void* p : dev) cudaFreeAsync(p, s);
+    cudaStreamSynchronize(s);
     for (void* p : host) cudaFreeHost(p);
     for (cudaEvent_t e : ev) cudaEventDestroy(e);
   }
   template <typename T> int dalloc(T** p, size_t bytes) {
     void* q = nullptr;
-    DFB_CUDA(h, cudaMalloc(&q, bytes ? bytes : 16));
+    DFB_CUDA(es, cudaMallocAsync(&q, bytes ? bytes : 16, s));
     dev.push_back(q);
     *p = static_cast<T*>(q);
     return 0;
   }
   template <typename T> int halloc(T** p, size_t bytes) {
     void* q = nullptr;
-    DFB_CUDA(h, cudaHostAlloc(&q, bytes ? bytes : 16, cudaHostAllocDefault));
+    DFB_CUDA(es, cudaHostAlloc(&q, bytes ? bytes : 16, cudaHostAllocDefault));
     host.push_back(q);
     *p = static_cast<T*>(q);
     return 0;
   }
   int event(cudaEvent_t* e) {
-    DFB_CUDA(h, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+    DFB_CUDA(es, cudaEventCreateWithFlags(e, cudaEventDisableTiming));
     ev.push_back(*e);
+    return 0;
+  }
+};
+
+// the writer's two pinned chunks and their events: a call's own (dfb_snapshot_write), or kept by a frozen copy
+// across its writes and freed at its release, off the writer thread
+struct PinnedChunks {
+  char* pin[2] = {nullptr, nullptr};
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  size_t bytes = 0;
+  PinnedChunks() = default;
+  PinnedChunks(const PinnedChunks&) = delete;
+  PinnedChunks& operator=(const PinnedChunks&) = delete;
+  ~PinnedChunks() { release(); }
+  void release() {
+    for (int i = 0; i < 2; ++i) {
+      if (pin[i]) cudaFreeHost(pin[i]);
+      if (ev[i]) cudaEventDestroy(ev[i]);
+      pin[i] = nullptr; ev[i] = nullptr;
+    }
+    bytes = 0;
+  }
+  int ensure(ErrSink* es, size_t chunk) {
+    if (chunk <= bytes) return 0;
+    release();
+    for (int i = 0; i < 2; ++i) {
+      DFB_CUDA(es, cudaHostAlloc(reinterpret_cast<void**>(&pin[i]), chunk, cudaHostAllocDefault));
+      DFB_CUDA(es, cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+    }
+    bytes = chunk;
     return 0;
   }
 };
@@ -89,26 +132,24 @@ struct Pass {
   size_t nk, bytes;
 };
 
-int snapshot_write(dfb_engine* h, int save_aux, size_t chunk, dfb_write_fn fn, void* ctx) {
-  const int k = h->prm.V_dim;
-  const bool aux = save_aux != 0;
-  DFB_TRY(drain(h));
-  TableState st;
-  DFB_TRY(read_state(h, &st));
-  Scratch sc(h);
-  cudaStream_t s = h->stream;
+// the v1 stream of table t (whose counts and InitV state are st) to fn, every pass on stream s.  Reads t and
+// nothing else of an engine: dfb_snapshot_write runs it over the live table between steps, dfb_frozen_write over a
+// frozen copy while steps run.  launches counts the kernels it ran.
+int write_records(const Table& t, const TableState& st, int k, bool aux, size_t chunk, dfb_write_fn fn, void* ctx,
+                  cudaStream_t s, PinnedChunks& pc, ErrSink* es, uint64_t* launches) {
+  Scratch sc(es, s);
   // ---- histogram: keys and V rows per bin of the top kCkptBinBits key bits ----
   const size_t nbins = size_t(1) << kCkptBinBits;
   unsigned *d_nk, *d_nv;
   DFB_TRY(sc.dalloc(&d_nk, nbins * 4));
   DFB_TRY(sc.dalloc(&d_nv, nbins * 4));
-  DFB_CUDA(h, cudaMemsetAsync(d_nk, 0, nbins * 4, s));
-  DFB_CUDA(h, cudaMemsetAsync(d_nv, 0, nbins * 4, s));
-  h->launches += launch_ckpt_hist(h->tab, d_nk, d_nv, s);
+  DFB_CUDA(es, cudaMemsetAsync(d_nk, 0, nbins * 4, s));
+  DFB_CUDA(es, cudaMemsetAsync(d_nv, 0, nbins * 4, s));
+  *launches += launch_ckpt_hist(t, d_nk, d_nv, s);
   std::vector<unsigned> nk(nbins), nv(nbins);
-  DFB_CUDA(h, cudaMemcpyAsync(nk.data(), d_nk, nbins * 4, cudaMemcpyDeviceToHost, s));
-  DFB_CUDA(h, cudaMemcpyAsync(nv.data(), d_nv, nbins * 4, cudaMemcpyDeviceToHost, s));
-  DFB_CUDA(h, cudaStreamSynchronize(s));
+  DFB_CUDA(es, cudaMemcpyAsync(nk.data(), d_nk, nbins * 4, cudaMemcpyDeviceToHost, s));
+  DFB_CUDA(es, cudaMemcpyAsync(nv.data(), d_nv, nbins * 4, cudaMemcpyDeviceToHost, s));
+  DFB_CUDA(es, cudaStreamSynchronize(s));
   // ---- passes: runs of consecutive bins whose records fit the staging budget (a larger single bin: one pass) ----
   const size_t fixed = fixed_bytes(aux), rowb = row_bytes(k, aux);
   const size_t budget = 4 * chunk;
@@ -128,7 +169,7 @@ int snapshot_write(dfb_engine* h, int save_aux, size_t chunk, dfb_write_fn fn, v
   }
   if (cur.nk) passes.push_back(cur);
   if (tk != st.n_keys || tv != st.n_vrows)
-    return h->fail(DFB_ERR_INVALID, "table changed while taking the snapshot");
+    return es->fail(DFB_ERR_INVALID, "table changed while taking the snapshot");
   size_t max_n = 0, max_bytes = 0;
   for (const Pass& p : passes) { max_n = std::max(max_n, p.nk); max_bytes = std::max(max_bytes, p.bytes); }
   // ---- header ----
@@ -136,7 +177,7 @@ int snapshot_write(dfb_engine* h, int save_aux, size_t chunk, dfb_write_fn fn, v
   memcpy(hd.magic, kSnapMagic, 8);
   hd.version = 1; hd.V_dim = k; hd.n_keys = st.n_keys; hd.n_vrows = st.n_vrows; hd.seed = st.seed;
   hd.has_aux = aux ? 1 : 0;
-  if (int rc = fn(ctx, &hd, sizeof(hd))) return h->fail(DFB_ERR_INVALID, "snapshot sink failed (" + std::to_string(rc) + ")");
+  if (int rc = fn(ctx, &hd, sizeof(hd))) return es->fail(DFB_ERR_INVALID, "snapshot sink failed (" + std::to_string(rc) + ")");
   if (passes.empty()) return 0;
   // ---- workspace of the largest pass, two pinned chunks ----
   CkptWs ws;
@@ -150,16 +191,13 @@ int snapshot_write(dfb_engine* h, int save_aux, size_t chunk, dfb_write_fn fn, v
   ws.tmp_bytes = ckpt_sort_tmp_bytes(max_n);
   DFB_TRY(sc.dalloc(&ws.tmp, ws.tmp_bytes));
   DFB_TRY(sc.dalloc(&ws.out, max_bytes));
-  char* pin[2];
-  cudaEvent_t ev[2];
-  for (int i = 0; i < 2; ++i) {
-    DFB_TRY(sc.halloc(&pin[i], chunk));
-    DFB_TRY(sc.event(&ev[i]));
-  }
+  DFB_TRY(pc.ensure(es, chunk));
+  char* const* pin = pc.pin;
+  const cudaEvent_t* ev = pc.ev;
   for (const Pass& p : passes) {
-    const int nl = launch_ckpt_pass(h->tab, p.b0, p.b1, p.nk, aux, k, ws, s);
-    if (nl < 0) return h->fail(DFB_ERR_CUDA, "snapshot pass failed (radix sort / scan)");
-    h->launches += nl;
+    const int nl = launch_ckpt_pass(t, p.b0, p.b1, p.nk, aux, k, ws, s);
+    if (nl < 0) return es->fail(DFB_ERR_CUDA, "snapshot pass failed (radix sort / scan)");
+    *launches += nl;
     // D2H of chunk c + 1 overlaps the sink call of chunk c
     const char* src = reinterpret_cast<const char*>(ws.out);
     const size_t nch = (p.bytes + chunk - 1) / chunk;
@@ -168,16 +206,23 @@ int snapshot_write(dfb_engine* h, int save_aux, size_t chunk, dfb_write_fn fn, v
       cudaMemcpyAsync(pin[c & 1], src + c * chunk, len, cudaMemcpyDeviceToHost, s);
       return cudaEventRecord(ev[c & 1], s);
     };
-    DFB_CUDA(h, issue(0));
+    DFB_CUDA(es, issue(0));
     for (size_t c = 0; c < nch; ++c) {
-      if (c + 1 < nch) DFB_CUDA(h, issue(c + 1));
-      DFB_CUDA(h, cudaEventSynchronize(ev[c & 1]));
+      if (c + 1 < nch) DFB_CUDA(es, issue(c + 1));
+      DFB_CUDA(es, cudaEventSynchronize(ev[c & 1]));
       const size_t len = std::min(chunk, p.bytes - c * chunk);
       if (int rc = fn(ctx, pin[c & 1], len))
-        return h->fail(DFB_ERR_INVALID, "snapshot sink failed (" + std::to_string(rc) + ")");
+        return es->fail(DFB_ERR_INVALID, "snapshot sink failed (" + std::to_string(rc) + ")");
     }
   }
-  DFB_CUDA(h, cudaGetLastError());
+  DFB_CUDA(es, cudaGetLastError());
+  return 0;
+}
+
+int check_chunk(size_t* chunk, ErrSink* es) {
+  if (*chunk == 0) *chunk = kDefaultChunk;
+  if (*chunk < sizeof(SnapHeader) || *chunk > kMaxChunk)
+    return es->fail(DFB_ERR_INVALID, "chunk_bytes must be 0 or in [40, 2^30]");
   return 0;
 }
 
@@ -194,8 +239,9 @@ int restore_read(dfb_engine* h, dfb_read_fn fn, void* ctx, uint32_t part, uint32
   TableState st;
   DFB_TRY(read_state(h, &st));
   const bool first = st.n_keys == 0 && h->restored_parts == 0;   // this stream's header seeds the InitV stream
-  Scratch sc(h);
   cudaStream_t s = h->stream;
+  ErrSink es{&h->err};
+  Scratch sc(&es, s);
   const size_t max_rec = std::max(fixed_bytes(true) + row_bytes(k, true), sizeof(SnapHeader));
   const size_t cap = chunk + max_rec;              // a chunk plus the carried-over start of a record
   const size_t max_n = cap / fixed_bytes(false) + 1;
@@ -343,6 +389,29 @@ size_t mem_read(void* ctx, void* buf, size_t cap) {
 
 }  // namespace
 
+// a snapshot frozen by dfb_snapshot_begin: a device copy of the table's slots and of its V rows, the table state at
+// that moment, and the writer's own low-priority stream, pinned chunks and error message
+struct dfb_frozen_s {
+  dfb_engine* h = nullptr;
+  int device = 0, V_dim = 0;
+  bool aux = false;
+  Table tab;
+  TableState st;
+  cudaStream_t stream = nullptr;
+  PinnedChunks chunks;
+  std::string err;
+  uint64_t launches = 0;
+};
+
+void dfbh::frozen_destroy(dfb_frozen_s* f) {
+  if (f->stream) {
+    dfbh::table_copy_free(&f->tab, f->stream);    // after the writer's last pass, without a device-wide wait
+    cudaStreamSynchronize(f->stream);
+    cudaStreamDestroy(f->stream);
+  }
+  delete f;
+}
+
 extern "C" {
 
 int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes) {
@@ -359,12 +428,61 @@ int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes) {
 int dfb_snapshot_write(dfb_handle h, int save_aux, size_t chunk_bytes, dfb_write_fn fn, void* ctx) {
   if (!h) return DFB_ERR_INVALID;
   if (!fn) return h->fail(DFB_ERR_INVALID, "write callback is NULL");
-  if (chunk_bytes == 0) chunk_bytes = kDefaultChunk;
-  if (chunk_bytes < sizeof(SnapHeader) || chunk_bytes > kMaxChunk)
-    return h->fail(DFB_ERR_INVALID, "chunk_bytes must be 0 or in [40, 2^30]");
+  ErrSink es{&h->err};
+  DFB_TRY(check_chunk(&chunk_bytes, &es));
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (save_aux && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data to save");
-  return snapshot_write(h, save_aux, chunk_bytes, fn, ctx);
+  DFB_TRY(drain(h));
+  TableState st;
+  DFB_TRY(read_state(h, &st));
+  PinnedChunks pc;
+  return write_records(h->tab, st, h->prm.V_dim, save_aux != 0, chunk_bytes, fn, ctx, h->stream, pc, &es,
+                       &h->launches);
+}
+
+int dfb_snapshot_begin(dfb_handle h, int save_aux, dfb_frozen* out) {
+  if (!h) return DFB_ERR_INVALID;
+  if (!out) return h->fail(DFB_ERR_INVALID, "out is NULL");
+  *out = nullptr;
+  if (h->frozen) return h->fail(DFB_ERR_INVALID, "the handle already has a frozen snapshot (release it first)");
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  if (save_aux && !h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data to save");
+  DFB_TRY(drain(h));
+  dfb_frozen_s* f = new dfb_frozen_s();
+  f->h = h; f->device = h->device; f->V_dim = h->prm.V_dim; f->aux = save_aux != 0;
+  if (int rc = read_state(h, &f->st)) { delete f; return rc; }
+  if (int rc = dfbh::table_copy(h, f->st.n_vrows, &f->tab)) { delete f; return rc; }
+  int least = 0, greatest = 0;
+  cudaError_t e = cudaDeviceGetStreamPriorityRange(&least, &greatest);
+  if (e == cudaSuccess) e = cudaStreamCreateWithPriority(&f->stream, cudaStreamNonBlocking, least);
+  if (e != cudaSuccess) {
+    dfbh::table_copy_free(&f->tab, h->stream);
+    delete f;
+    return h->cuda_fail(e, "cudaStreamCreateWithPriority(frozen snapshot)");
+  }
+  h->frozen = f;
+  *out = f;
+  return DFB_OK;
+}
+
+int dfb_frozen_write(dfb_frozen f, size_t chunk_bytes, dfb_write_fn fn, void* ctx) {
+  if (!f) return DFB_ERR_INVALID;
+  ErrSink es{&f->err};
+  if (!fn) return es.fail(DFB_ERR_INVALID, "write callback is NULL");
+  DFB_TRY(check_chunk(&chunk_bytes, &es));
+  DFB_CUDA(&es, cudaSetDevice(f->device));
+  return write_records(f->tab, f->st, f->V_dim, f->aux, chunk_bytes, fn, ctx, f->stream, f->chunks, &es,
+                       &f->launches);
+}
+
+const char* dfb_frozen_error(dfb_frozen f) { return f ? f->err.c_str() : "frozen snapshot is NULL"; }
+
+int dfb_frozen_release(dfb_frozen f) {
+  if (!f) return DFB_OK;
+  cudaSetDevice(f->device);
+  f->h->frozen = nullptr;
+  dfbh::frozen_destroy(f);
+  return DFB_OK;
 }
 
 int dfb_restore_read(dfb_handle h, dfb_read_fn fn, void* ctx, uint32_t part, uint32_t nparts, uint32_t shard,

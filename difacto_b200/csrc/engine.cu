@@ -773,6 +773,8 @@ int dfb_destroy(dfb_handle h) {
   if (!h) return DFB_OK;
   cudaSetDevice(h->device);
   cudaDeviceSynchronize();
+  if (h->frozen) dfbh::frozen_destroy(h->frozen);   // a frozen snapshot not released: its handle dangles from here
+  h->frozen = nullptr;
   if (h->shard) dfbh::shard_destroy(h);
   for (auto& L : h->loc) {
     DevBuf* lb[] = {&L.keys, &L.lidx, &L.cnt, &L.occ_sorted, &L.col_start, &L.col_end, &L.scal};
@@ -848,6 +850,30 @@ int dfb_rng_state(dfb_handle h, uint32_t* seed) {
   DFB_CUDA(h, cudaMemcpyAsync(&st, h->tab.state, sizeof(st), cudaMemcpyDeviceToHost, h->stream));
   DFB_CUDA(h, cudaStreamSynchronize(h->stream));
   *seed = st.seed;
+  return DFB_OK;
+}
+
+int dfb_id_range_get(dfb_handle h, int* bits) {
+  if (!h || !bits) return DFB_ERR_INVALID;
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  // the key masks of the batches enqueued so far widen the range once read: wait for them and fold them in
+  for (int q = 0; q < 2; ++q)
+    if (h->or_pending[q]) {
+      DFB_CUDA(h, cudaEventSynchronize(h->ev_or[q]));
+      h->or_pending[q] = false;
+      const int b = lowest_bit(h->h_or[q]);
+      if (h->loc_begin_bit < 0 || b < h->loc_begin_bit) h->loc_begin_bit = b;
+    }
+  *bits = h->loc_begin_bit < 0 ? 0 : 64 - h->loc_begin_bit;
+  return DFB_OK;
+}
+
+int dfb_id_range_set(dfb_handle h, int bits) {
+  if (!h) return DFB_ERR_INVALID;
+  if (bits < 1 || bits > 64) return h->fail(DFB_ERR_INVALID, "id range bits must be in [1, 64]");
+  if (h->loc_begin_bit >= 0 || h->or_pending[0] || h->or_pending[1])
+    return h->fail(DFB_ERR_INVALID, "the engine has already learned an id range");
+  h->loc_begin_bit = 64 - bits;
   return DFB_OK;
 }
 

@@ -17,6 +17,7 @@ struct DevBuf {
 };
 
 struct ShardState;   // shard.cu
+struct dfb_frozen_s; // checkpoint.cu
 
 struct dfb_engine {
   dfb::Params prm;
@@ -99,6 +100,7 @@ struct dfb_engine {
   dfb::DevProgress* h_prog = nullptr;   // pinned
   unsigned long long* h_nvals = nullptr;  // pinned
   ShardState* shard = nullptr;          // the NVLink-sharded store this engine is a rank of (shard.cu)
+  dfb_frozen_s* frozen = nullptr;       // the snapshot dfb_snapshot_begin froze, until dfb_frozen_release
 
   // capacity growth up to table_capacity_max / V_capacity_max (growth.cu)
   struct Growth {
@@ -193,6 +195,12 @@ void capacity_destroy(dfb_engine* h);
 // waits for the device, and a failed allocation keeps the current table and pool (a step that really overflows them
 // reports DFB_ERR_CAPACITY).  Does nothing on an engine that cannot grow.
 int reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows);
+// a copy of the table's slots (cap entries) and of V rows [0, n_vrows) in fresh stream-ordered device memory, made
+// on h->stream and waited for; DFB_ERR_CAPACITY with nothing allocated when the memory cannot be had.  The copy keeps
+// cap, mask, ks and rs, has vcap = n_vrows and no state or progress: the snapshot writer's view of a table.
+int table_copy(dfb_engine* h, uint64_t n_vrows, dfb::Table* out);
+void table_copy_free(dfb::Table* t, cudaStream_t s);   // stream-ordered on s
+void frozen_destroy(dfb_frozen_s* f);   // checkpoint.cu: frees the copy after its stream's work
 void shard_destroy(dfb_engine* h);      // shard.cu
 int shard_sync(dfb_engine* h);          // shard.cu: drain the shard's streams
 }  // namespace dfbh

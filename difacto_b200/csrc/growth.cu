@@ -225,3 +225,49 @@ int dfbh::reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows) {
   g.total_v += new_vrows;
   return 0;
 }
+
+int dfbh::table_copy(dfb_engine* h, uint64_t n_vrows, Table* out) {
+  const Table& t = h->tab;
+  Table c = t;
+  c.V = c.Vcg = nullptr;
+  c.vcap = n_vrows;
+  c.state = nullptr; c.prog = nullptr;
+  const size_t vbytes = (size_t)n_vrows * row_bytes(h);
+  cudaStream_t s = h->stream;
+  // an engine that can still grow keeps room for that growth: the copy is refused (the caller falls back to the
+  // blocking writer) rather than starving a later rehash or pool mapping into DFB_ERR_CAPACITY
+  const dfb_engine::Growth& g = h->grow;
+  if (g.on) {
+    size_t need = t.cap * sizeof(Entry) + vbytes;
+    if (t.max_keys < g.tab_max) need += next_pow2(2 * g.tab_max) * sizeof(Entry) * 3 / 2;  // the last rehash: new + old
+    if (g.vbase) need += std::min(round_up((size_t)g.v_max * row_bytes(h), g.gran), g.vreserved) - g.vmapped;
+    size_t free_b = 0, total_b = 0;
+    DFB_CUDA(h, cudaMemGetInfo(&free_b, &total_b));
+    if (free_b < need)
+      return h->fail(DFB_ERR_CAPACITY, "no device memory for a copy of the table beside the growth up to "
+                                       "table_capacity_max / V_capacity_max");
+  }
+  if (cudaMallocAsync(reinterpret_cast<void**>(&c.tab), t.cap * sizeof(Entry), s) != cudaSuccess) {
+    cudaGetLastError();
+    return h->fail(DFB_ERR_CAPACITY, "no device memory for a copy of the table");
+  }
+  if (vbytes && cudaMallocAsync(reinterpret_cast<void**>(&c.V), vbytes, s) != cudaSuccess) {
+    cudaGetLastError();
+    cudaFreeAsync(c.tab, s);
+    cudaStreamSynchronize(s);
+    return h->fail(DFB_ERR_CAPACITY, "no device memory for a copy of the V rows");
+  }
+  if (c.V) c.Vcg = c.V + t.ks;
+  DFB_CUDA(h, cudaMemcpyAsync(c.tab, t.tab, t.cap * sizeof(Entry), cudaMemcpyDeviceToDevice, s));
+  if (vbytes) DFB_CUDA(h, cudaMemcpyAsync(c.V, t.V, vbytes, cudaMemcpyDeviceToDevice, s));
+  // the sharded store inserts on streams of its own: the copy is complete before any later step may run
+  DFB_CUDA(h, cudaStreamSynchronize(s));
+  *out = c;
+  return 0;
+}
+
+void dfbh::table_copy_free(Table* t, cudaStream_t s) {
+  if (t->tab) cudaFreeAsync(t->tab, s);
+  if (t->V) cudaFreeAsync(t->V, s);
+  t->tab = nullptr; t->V = t->Vcg = nullptr;
+}

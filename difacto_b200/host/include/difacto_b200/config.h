@@ -90,6 +90,10 @@ struct SGDLearnerParam {
                              // and one table shard per GPU, dfb_shard_*; needs fused = 1)
   long long shard_max_nnz = 0;   // engine-only: capacity (non-zeros) of one minibatch in the sharded store;
                                  // 0 = batch_size * 256
+  // engine-only: a checkpoint every checkpoint_period training minibatches per worker (0: none) into
+  // checkpoint_out.<c>.* and the pointer file checkpoint_out; checkpoint_in resumes the run a pointer file names
+  std::string checkpoint_out, checkpoint_in;
+  long long checkpoint_period = 0;
 
   KWArgs InitAllowUnknown(const KWArgs& kwargs) {
     KWArgs remain;
@@ -114,6 +118,9 @@ struct SGDLearnerParam {
         else if (k == "fused") fused = std::stoi(v);
         else if (k == "num_gpus") num_gpus = std::stoi(v);
         else if (k == "shard_max_nnz") shard_max_nnz = std::stoll(v);
+        else if (k == "checkpoint_out") checkpoint_out = v;
+        else if (k == "checkpoint_in") checkpoint_in = v;
+        else if (k == "checkpoint_period") checkpoint_period = std::stoll(v);
         else remain.push_back(kv);
       } catch (const std::logic_error&) {
         throw ParamError("Invalid Parameter format for " + k + " value='" + v + "'");
@@ -121,6 +128,8 @@ struct SGDLearnerParam {
     }
     if (!has_data_in) throw ParamError("Required parameter data_in of string is not presented");
     if (batch_size < 0) throw ParamError("Required parameter batch_size of int is not presented");   // sgd_param.h:58
+    if (checkpoint_period < 0) throw ParamError("checkpoint_period must be >= 0");
+    if (checkpoint_period > 0 && checkpoint_out.empty()) throw ParamError("checkpoint_period needs checkpoint_out");
     return remain;
   }
 };

@@ -18,9 +18,11 @@
 #include <memory>
 #include <mutex>
 #include <string>
+#include <thread>
 #include <vector>
 
 #include "api.h"
+#include "checkpoint_state.h"
 #include "config.h"
 #include "data.h"
 #include "engine_adapters.h"
@@ -53,7 +55,7 @@ class SGDLearner : public Learner {
  public:
   typedef std::function<void(int epoch, const sgd::Progress& train, const sgd::Progress& val)> EpochCallback;
   SGDLearner() {}
-  ~SGDLearner() override { delete loss_; delete store_; }
+  ~SGDLearner() override;
   KWArgs Init(const KWArgs& kwargs) override;
   void AddEpochEndCallback(const EpochCallback& cb) { epoch_end_callback_.push_back(cb); }
   GpuSGDUpdater* GetUpdater() { return static_cast<GpuSGDUpdater*>(store_->updater().get()); }
@@ -74,7 +76,15 @@ class SGDLearner : public Learner {
   /** num_gpus > 1: one epoch over all N * num_jobs_per_epoch file parts, part i handled by worker i % N.
    * pred_out (task=predict): predict steps, and the predictions of every row to that file, in file order */
   void RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, const std::string* pred_out = nullptr);
-  void LoadShards();
+  /** the model X (one file) or X_part-0 .. of a num_gpus = M run into the engines (model_in, checkpoint_in) */
+  void LoadShards(const std::string& base);
+  /** checkpoint_in: the model, the id ranges and the position in the run of the checkpoint the pointer file names */
+  void LoadCheckpoint();
+  /** after a training minibatch per worker: a checkpoint when the period has come round.  The model is frozen on
+   * every GPU now; a helper thread writes it, then the state record, then renames the pointer file */
+  void MaybeCheckpoint();
+  /** waits for the checkpoint write in flight and releases its device copies; throws what it failed with */
+  void WaitCheckpoint();
   /** engine of GPU r (r = 0: the updater's own) */
   const std::shared_ptr<GpuEngine>& ShardEngine(int r) { return r == 0 ? GetUpdater()->engine() : shard_engines_[r - 1]; }
   void BatchFused(const RowBlockContainer<unsigned>& data, const std::vector<feaid_t>& keys,
@@ -89,6 +99,18 @@ class SGDLearner : public Learner {
   SGDLearnerParam param_;
   std::vector<EpochCallback> epoch_end_callback_;
   std::vector<std::shared_ptr<GpuEngine>> shard_engines_;     // GPUs 1..N-1 (num_gpus > 1)
+
+  // checkpoints: the settings the state record fingerprints, the run's position (kept current by the drivers), the
+  // state to resume from, and the write in flight
+  std::vector<std::pair<std::string, std::string>> settings_;
+  CheckpointState pos_;
+  sgd::Progress* epoch_prog_ = nullptr;   // the Progress of the epoch being trained, and (num_gpus = 1) of its part
+  sgd::Progress* part_prog_ = nullptr;
+  std::unique_ptr<CheckpointState> resume_;
+  int ckpt_seq_ = 0, ckpt_prev_ = -1;
+  std::thread ckpt_thread_;
+  std::string ckpt_error_;
+  std::vector<dfb_frozen> frozen_;
 };
 
 }  // namespace difacto

@@ -2,10 +2,16 @@
 // src/sgd/sgd_learner.cc of the reference (cited per function); the arithmetic lives on the GPU.
 #include "difacto_b200/sgd_learner.h"
 
+#include <errno.h>
+#include <fcntl.h>
+#include <unistd.h>
+
 #include <cstdint>
 #include <cstdio>
+#include <cstdlib>
 #include <cstring>
 #include <fstream>
+#include <sstream>
 #include <thread>
 
 namespace difacto {
@@ -24,9 +30,55 @@ Learner* Learner::Create(const std::string& type) {   // src/learner.cc:15-26
   throw Error("unknown learner type: " + type + " (the GPU engine accelerates the sgd learner)");
 }
 
+namespace {
+// a setting as the engine parses it: a float as the float it parses to (%.9g tells every float apart), an integer as
+// that integer.  Anything else as given (the engine refuses it).
+std::string FloatSetting(float f) {
+  char b[64];
+  snprintf(b, sizeof(b), "%.9g", f);
+  return b;
+}
+std::string FloatSetting(const std::string& v) {
+  char* end = nullptr;
+  const float f = strtof(v.c_str(), &end);
+  if (v.empty() || *end) return v;
+  return FloatSetting(f);
+}
+std::string IntSetting(const std::string& v) {
+  char* end = nullptr;
+  const long long x = strtoll(v.c_str(), &end, 10);
+  if (v.empty() || *end) return v;
+  return std::to_string(x);
+}
+}  // namespace
+
+SGDLearner::~SGDLearner() {
+  if (ckpt_thread_.joinable()) ckpt_thread_.join();
+  for (dfb_frozen f : frozen_) if (f) dfb_frozen_release(f);
+  delete loss_;
+  delete store_;
+}
+
 // SGDLearner::Init, sgd_learner.cc:229-246
 KWArgs SGDLearner::Init(const KWArgs& kwargs) {
   KWArgs remain = param_.InitAllowUnknown(kwargs);
+  // what fixes the minibatches and the model: a checkpoint resumes only under the same settings
+  settings_ = {{"data_in", param_.data_in}, {"data_val", param_.data_val}, {"data_format", param_.data_format},
+               {"loss", param_.loss}, {"num_gpus", std::to_string(param_.num_gpus)},
+               {"num_jobs_per_epoch", std::to_string(param_.num_jobs_per_epoch)},
+               {"batch_size", std::to_string(param_.batch_size)}, {"shuffle", std::to_string(param_.shuffle)},
+               {"neg_sampling", FloatSetting(param_.neg_sampling)}};
+  // SGDUpdaterParam (sgd_param.h:94-106) and id_bits, with the engine's defaults for the keys not given
+  struct Key { const char* name; const char* dflt; bool is_float; };
+  const Key keys[] = {{"l1", "1", true}, {"l2", "0", true}, {"V_l2", ".01", true}, {"lr", ".01", true},
+                      {"lr_beta", "1", true}, {"V_lr", ".01", true}, {"V_lr_beta", "1", true},
+                      {"V_init_scale", ".01", true}, {"V_dim", "-1", false}, {"V_threshold", "10", false},
+                      {"seed", "0", false}, {"id_bits", "0", false}};
+  for (const Key& k : keys) {
+    std::string v = k.dflt;
+    for (const auto& kv : kwargs) if (kv.first == k.name) v = kv.second;
+    settings_.push_back(std::make_pair(std::string(k.name), k.is_float ? FloatSetting(v) : IntSetting(v)));
+  }
   auto* updater = new GpuSGDUpdater();
   std::shared_ptr<Updater> holder(updater);
   remain = updater->Init(remain);
@@ -81,8 +133,7 @@ void KeyRange(uint32_t r, uint32_t S, uint64_t* lo, uint64_t* hi) {
 // of a num_gpus = M run.  num_gpus = 1 reads X when it exists, otherwise the parts; num_gpus = N > 1 reads the parts
 // when X_part-0 exists, otherwise X.  Rank r of N restores every part whose key range overlaps its own and keeps its
 // keys (dfb_restore_read), so M parts load into any number of GPUs; M = N is part r alone.
-void SGDLearner::LoadShards() {
-  const std::string& base = param_.model_in;
+void SGDLearner::LoadShards(const std::string& base) {
   auto part_name = [&](int p) { return base + "_part-" + std::to_string(p); };
   const bool parts = param_.num_gpus > 1 ? FileExists(part_name(0)) : !FileExists(base);
   std::vector<std::string> files;
@@ -120,8 +171,14 @@ void SGDLearner::LoadShards() {
 void SGDLearner::RunScheduler() {
   // num_gpus = N > 1: one snapshot per shard, <name>_part-<r> (the format of Updater::Save per shard)
   auto shard_name = [&](const std::string& base, int r) { return param_.num_gpus > 1 ? base + "_part-" + std::to_string(r) : base; };
-  if (!param_.model_in.empty()) LoadShards();
+  if (!param_.checkpoint_in.empty()) {
+    if (!param_.model_in.empty()) throw ParamError("checkpoint_in and model_in both load a model: give one of them");
+    LoadCheckpoint();
+  } else if (!param_.model_in.empty()) {
+    LoadShards(param_.model_in);
+  }
   RunEpochs();
+  WaitCheckpoint();
   if (!param_.model_out.empty()) {
     for (int r = 0; r < param_.num_gpus; ++r) {
       const std::string fn = shard_name(param_.model_out, r);
@@ -171,14 +228,14 @@ sgd::Progress SGDLearner::Predict() {
   if (param_.model_in.empty()) throw Error("task=predict needs model_in");
   if (param_.num_gpus > 1) {
     // the model (one file or any number of parts), re-sharded over and scored by N GPUs
-    LoadShards();
+    LoadShards(param_.model_in);
     sgd::Progress prog;
     param_.data_val = param_.data_in;
     RunEpochSharded(0, sgd::Job::kValidation, &prog, param_.pred_out.empty() ? nullptr : &param_.pred_out);
     if (verbose) printf(" - Prediction: %s, rows = %g\n", prog.TextString().c_str(), prog.nrows);
     return prog;
   }
-  LoadShards();      // one file, or all parts of a num_gpus = M model merged into this GPU
+  LoadShards(param_.model_in);      // one file, or all parts of a num_gpus = M model merged into this GPU
   FILE* fo = param_.pred_out.empty() ? nullptr : fopen(param_.pred_out.c_str(), "w");
   if (!param_.pred_out.empty() && !fo) throw Error("failed to open pred_out " + param_.pred_out);
   sgd::Progress prog;
@@ -221,10 +278,30 @@ sgd::Progress SGDLearner::Predict() {
   return prog;
 }
 
+namespace {
+void ToBits(const sgd::Progress& p, float* out) {
+  out[0] = p.loss; out[1] = p.penalty; out[2] = p.auc; out[3] = p.nnz_w; out[4] = p.nrows;
+}
+sgd::Progress FromBits(const float* in) {
+  sgd::Progress p;
+  p.loss = in[0]; p.penalty = in[1]; p.auc = in[2]; p.nnz_w = in[3]; p.nrows = in[4];
+  return p;
+}
+}  // namespace
+
 void SGDLearner::RunEpochs() {
-  real_t pre_loss = 0, pre_val_auc = 0;
-  for (int k = 0; k < param_.max_num_epochs; ++k) {
+  real_t& pre_loss = pos_.pre_loss;
+  real_t& pre_val_auc = pos_.pre_val_auc;
+  pre_loss = 0; pre_val_auc = 0;
+  int k0 = 0;
+  if (resume_) {        // the epoch the checkpoint was taken in, and what the finished part of it added up to
+    k0 = resume_->epoch;
+    pre_loss = resume_->pre_loss;
+    pre_val_auc = resume_->pre_val_auc;
+  }
+  for (int k = k0; k < param_.max_num_epochs; ++k) {
     sgd::Progress train_prog, val_prog;
+    if (resume_) train_prog = FromBits(resume_->epoch_prog);
     if (verbose) printf("Start epoch %d\n", k);
     RunEpoch(k, sgd::Job::kTraining, &train_prog);
     if (verbose) printf(" - Training: %s\n", train_prog.TextString().c_str());
@@ -257,13 +334,23 @@ void SGDLearner::RunEpochs() {
 void SGDLearner::RunEpoch(int epoch, int job_type, sgd::Progress* prog) {
   if (param_.num_gpus > 1) { RunEpochSharded(epoch, job_type, prog); return; }
   const int n = store_->NumWorkers() * param_.num_jobs_per_epoch;
-  for (int i = 0; i < n; ++i) {
+  const bool train = job_type == sgd::Job::kTraining;
+  int i0 = 0;
+  sgd::Progress p0;
+  if (train && resume_) {      // resumed: from the part the checkpoint was taken in, with its Progress so far
+    i0 = resume_->workers[0].part;
+    p0 = FromBits(resume_->part_prog);
+  }
+  for (int i = i0; i < n; ++i) {
     sgd::Job job;
     job.type = job_type; job.epoch = epoch; job.num_parts = n; job.part_idx = i;
-    sgd::Progress p;
+    sgd::Progress p = i == i0 ? p0 : sgd::Progress();
+    epoch_prog_ = prog;
+    part_prog_ = &p;
     IterateData(job, &p);
     prog->Merge(p);
   }
+  epoch_prog_ = part_prog_ = nullptr;
 }
 
 // num_gpus = N > 1: the epoch of sgd_learner.cc:70-111 with N workers.  File part i of the N * num_jobs_per_epoch
@@ -290,12 +377,17 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
   };
   struct Worker {
     int part = 0;
+    uint64_t consumed = 0, skip = 0;     // minibatches read from the part; and still to be replayed on a resume
     std::unique_ptr<BatchReader> reader;
     bool has = false;
     std::string error;
   };
   std::vector<Worker> w(N);
   for (int r = 0; r < N; ++r) w[r].part = r;
+  if (train && resume_) {      // resumed: each worker on its part, past the minibatches it had read
+    for (int r = 0; r < N; ++r) { w[r].part = resume_->workers[r].part; w[r].skip = resume_->workers[r].consumed; }
+    resume_.reset();
+  }
   auto next = [&](int r) {          // host only (file parsing): runs on a helper thread per worker
     Worker& me = w[r];
     me.has = false;
@@ -308,8 +400,11 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
                                           train ? static_cast<unsigned>(param_.batch_size) : 65536u,
                                           train ? static_cast<unsigned>(param_.batch_size) * static_cast<unsigned>(param_.shuffle) : 0u,
                                           train ? param_.neg_sampling : 1.0f, static_cast<unsigned>(epoch)));
+          me.consumed = 0;
+          for (; me.skip; --me.skip, ++me.consumed)    // read and dropped on the host: the GPUs had them
+            if (!me.reader->Next()) throw Error("checkpoint_in: file part " + std::to_string(me.part) + " is shorter than the checkpoint says");
         }
-        if (me.reader->Next()) { me.has = true; return; }
+        if (me.reader->Next()) { me.has = true; ++me.consumed; return; }
         me.reader.reset();
         me.part += N;
       }
@@ -359,6 +454,16 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
         const size_t n = w[r].reader->Value().size;
         WritePreds(f, pred_bufs[r].get<real_t>(n ? n : 1), n);
       }
+    }
+    if (train) {     // every rank's checkpoint after the same collected round
+      pos_.epoch = epoch;
+      pos_.has_rand = false;
+      pos_.workers.resize(N);
+      for (int r = 0; r < N; ++r) { pos_.workers[r].part = w[r].part; pos_.workers[r].consumed = w[r].consumed; }
+      epoch_prog_ = prog;
+      part_prog_ = nullptr;
+      MaybeCheckpoint();
+      epoch_prog_ = nullptr;
     }
   }
   if (!predict) return;
@@ -459,6 +564,11 @@ void SGDLearner::BatchPluginCalls(const RowBlockContainer<unsigned>& data_c, con
 // SGDLearner::IterateData, sgd_learner.cc:129-227
 void SGDLearner::IterateData(const sgd::Job& job, sgd::Progress* progress) {
   const bool train = job.type == sgd::Job::kTraining;
+  // the reader draws its shuffle from rand(): a resume restores it as it was at the start of the part, and every
+  // checkpoint records it so
+  if (train && resume_ && resume_->has_rand) resume_->rand.Restore();
+  RandState rand_at_start;
+  if (train && param_.checkpoint_period > 0) rand_at_start = RandState::Save();
   // training: BatchReader(batch_size, shuffle window = batch_size*shuffle, neg_sampling) (:182-188);
   // validation: plain reader, here in chunks of 65536 rows (:190-194 reads 256 MB chunks)
   BatchReader reader(train ? param_.data_in : param_.data_val, param_.data_format,
@@ -467,7 +577,24 @@ void SGDLearner::IterateData(const sgd::Job& job, sgd::Progress* progress) {
                      train ? static_cast<unsigned>(param_.batch_size) * static_cast<unsigned>(param_.shuffle) : 0u,
                      train ? param_.neg_sampling : 1.0f, static_cast<unsigned>(job.epoch), 0,
                      ShuffleOrder::kReference);      // one reader at a time: the reference's own shuffle order
+  uint64_t skip = 0;
+  if (train) {
+    pos_.epoch = job.epoch;
+    pos_.workers.assign(1, CheckpointState::Worker());
+    pos_.workers[0].part = job.part_idx;
+    pos_.has_rand = param_.checkpoint_period > 0;
+    pos_.rand = rand_at_start;
+  }
+  if (train && resume_) {
+    skip = resume_->workers[0].consumed;
+    resume_.reset();
+  }
   while (reader.Next()) {
+    if (skip) {        // resumed: the minibatches the checkpoint had trained, read and dropped on the host
+      --skip;
+      ++pos_.workers[0].consumed;
+      continue;
+    }
     const bool push_cnt = train && job.epoch == 0;   // :201-202
     if (param_.fused == 1) {
       // Localizer::Compact + [kFeaCount push] + Pull/Predict/.../Push in one device call on the raw block
@@ -478,16 +605,181 @@ void SGDLearner::IterateData(const sgd::Job& job, sgd::Progress* progress) {
                                     blk.index, blk.value, blk.label, push_cnt ? 1 : 0, train ? 1 : 0, &pr, nullptr),
                  "dfb_train_step_raw");
       progress->loss += pr.loss; progress->penalty += pr.penalty; progress->auc += pr.auc; progress->nrows += pr.nrows;
-      continue;
+    } else {
+      RowBlockContainer<unsigned> data;
+      std::vector<feaid_t> feaids;
+      std::vector<real_t> feacnt;
+      Localizer lc(-1, 2);
+      lc.Compact(reader.Value(), &data, &feaids, push_cnt ? &feacnt : nullptr);
+      if (param_.fused == 2) BatchFused(data, feaids, push_cnt ? &feacnt : nullptr, train, progress);
+      else BatchPluginCalls(data, feaids, push_cnt ? &feacnt : nullptr, train, progress);
     }
-    RowBlockContainer<unsigned> data;
-    std::vector<feaid_t> feaids;
-    std::vector<real_t> feacnt;
-    Localizer lc(-1, 2);
-    lc.Compact(reader.Value(), &data, &feaids, push_cnt ? &feacnt : nullptr);
-    if (param_.fused == 2) BatchFused(data, feaids, push_cnt ? &feacnt : nullptr, train, progress);
-    else BatchPluginCalls(data, feaids, push_cnt ? &feacnt : nullptr, train, progress);
+    if (train) {
+      ++pos_.workers[0].consumed;
+      MaybeCheckpoint();
+    }
   }
+}
+
+namespace {
+// dfb_write_fn into a file descriptor
+int FdSink(void* ctx, const void* buf, size_t bytes) {
+  const int fd = *static_cast<const int*>(ctx);
+  const char* p = static_cast<const char*>(buf);
+  while (bytes) {
+    const ssize_t n = ::write(fd, p, bytes);
+    if (n < 0) {
+      if (errno == EINTR) continue;
+      return 1;
+    }
+    p += n;
+    bytes -= static_cast<size_t>(n);
+  }
+  return 0;
+}
+
+// path, filled by fill(fd), then flushed to the disk
+void WriteSynced(const std::string& path, const std::function<void(int)>& fill) {
+  const int fd = ::open(path.c_str(), O_WRONLY | O_CREAT | O_TRUNC, 0644);
+  if (fd < 0) throw Error("failed to open " + path + ": " + strerror(errno));
+  try {
+    fill(fd);
+  } catch (...) {
+    ::close(fd);
+    throw;
+  }
+  const bool synced = ::fsync(fd) == 0;
+  if (::close(fd) != 0 || !synced) throw Error("failed to write " + path + ": " + strerror(errno));
+}
+
+void WriteBytes(const std::string& path, const std::string& bytes) {
+  WriteSynced(path, [&](int fd) {
+    if (FdSink(&fd, bytes.data(), bytes.size())) throw Error("failed to write " + path + ": " + strerror(errno));
+  });
+}
+
+// the directory entry of a rename, flushed to the disk
+void SyncDir(const std::string& path) {
+  const size_t slash = path.rfind('/');
+  const std::string dir = slash == std::string::npos ? "." : (slash == 0 ? "/" : path.substr(0, slash));
+  const int fd = ::open(dir.c_str(), O_RDONLY | O_DIRECTORY);
+  if (fd < 0) return;
+  ::fsync(fd);
+  ::close(fd);
+}
+
+// the model file of rank r in checkpoint `base` (= P.<c>): the names model_out / model_in use
+std::string CkptModel(const std::string& base, int N, int r) {
+  return N > 1 ? base + ".model_part-" + std::to_string(r) : base + ".model";
+}
+
+void RemoveCheckpoint(const std::string& P, int c, int N) {
+  const std::string base = P + "." + std::to_string(c);
+  for (int r = 0; r < N; ++r) std::remove(CkptModel(base, N, r).c_str());
+  std::remove((base + ".state").c_str());
+}
+}  // namespace
+
+// checkpoint c: P.<c>.model (P.<c>.model_part-<r>), P.<c>.state, then P names c.  Until the rename, P names c - 1,
+// which stays complete on the disk; it is removed after.
+void SGDLearner::MaybeCheckpoint() {
+  ++pos_.minibatches;
+  if (param_.checkpoint_period <= 0 || pos_.minibatches % static_cast<uint64_t>(param_.checkpoint_period) != 0) return;
+  WaitCheckpoint();
+  const int N = param_.num_gpus;
+  const int c = ckpt_seq_++;
+  const std::string P = param_.checkpoint_out, base = P + "." + std::to_string(c);
+  CheckpointState st = pos_;
+  st.settings = settings_;
+  ToBits(*epoch_prog_, st.epoch_prog);
+  if (part_prog_) ToBits(*part_prog_, st.part_prog);
+  st.id_ranges.assign(N, 0);
+  for (int r = 0; r < N; ++r) ShardEngine(r)->Check(dfb_id_range_get(ShardEngine(r)->handle(), &st.id_ranges[r]), "dfb_id_range_get");
+  // freeze every rank's model on its GPU; where there is no room for the copy, write that rank's model now
+  frozen_.assign(N, nullptr);
+  for (int r = 0; r < N; ++r) {
+    const auto& e = ShardEngine(r);
+    const int rc = dfb_snapshot_begin(e->handle(), 1, &frozen_[r]);
+    if (rc == DFB_ERR_CAPACITY) {
+      frozen_[r] = nullptr;
+      WriteSynced(CkptModel(base, N, r), [&](int fd) {
+        e->Check(dfb_snapshot_write(e->handle(), 1, 0, FdSink, &fd), "dfb_snapshot_write");
+      });
+    } else {
+      e->Check(rc, "dfb_snapshot_begin");
+    }
+  }
+  const std::string rec = st.Serialize();
+  if (verbose) {
+    printf("Checkpoint %d: minibatch %llu, epoch %d, part:minibatches", c, static_cast<unsigned long long>(st.minibatches),
+           st.epoch);
+    for (const auto& w : st.workers) printf(" %d:%llu", w.part, static_cast<unsigned long long>(w.consumed));
+    printf("\n");
+  }
+  const int prev = ckpt_prev_;
+  ckpt_prev_ = c;
+  const std::vector<dfb_frozen> fr = frozen_;
+  ckpt_thread_ = std::thread([this, fr, rec, P, base, c, prev, N]() {
+    try {
+      for (int r = 0; r < N; ++r) {
+        if (!fr[r]) continue;
+        WriteSynced(CkptModel(base, N, r), [&](int fd) {
+          if (dfb_frozen_write(fr[r], 0, FdSink, &fd) != DFB_OK)
+            throw Error(std::string("dfb_frozen_write: ") + dfb_frozen_error(fr[r]));
+        });
+      }
+      WriteBytes(base + ".state", rec);
+      const std::string tmp = P + ".tmp";
+      WriteBytes(tmp, std::to_string(c) + "\n");
+      if (std::rename(tmp.c_str(), P.c_str()) != 0) throw Error("failed to rename " + tmp + " to " + P);
+      SyncDir(P);
+      if (prev >= 0) RemoveCheckpoint(P, prev, N);
+    } catch (const std::exception& e) {
+      ckpt_error_ = e.what();
+    }
+  });
+}
+
+void SGDLearner::WaitCheckpoint() {
+  if (ckpt_thread_.joinable()) ckpt_thread_.join();
+  for (dfb_frozen f : frozen_) if (f) dfb_frozen_release(f);
+  frozen_.clear();
+  if (!ckpt_error_.empty()) {
+    std::string e;
+    e.swap(ckpt_error_);
+    throw Error("checkpoint: " + e);
+  }
+}
+
+void SGDLearner::LoadCheckpoint() {
+  const std::string& P = param_.checkpoint_in;
+  std::ifstream fp(P);
+  if (!fp) throw Error("checkpoint_in: failed to open " + P);
+  long long c = -1;
+  fp >> c;
+  if (!fp || c < 0) throw Error("checkpoint_in: " + P + " does not name a checkpoint");
+  const std::string base = P + "." + std::to_string(c);
+  std::ifstream fs(base + ".state", std::ios::binary);
+  if (!fs) throw Error("checkpoint_in: checkpoint " + std::to_string(c) + " that " + P + " names is missing (" + base + ".state)");
+  std::stringstream ss;
+  ss << fs.rdbuf();
+  std::unique_ptr<CheckpointState> st(new CheckpointState(CheckpointState::Parse(ss.str())));
+  st->CheckSettings(settings_);
+  const int N = param_.num_gpus;
+  if (static_cast<int>(st->workers.size()) != N || static_cast<int>(st->id_ranges.size()) != N)
+    throw Error("checkpoint_in: " + base + ".state does not hold " + std::to_string(N) + " workers");
+  for (int r = 0; r < N; ++r)
+    if (!FileExists(CkptModel(base, N, r)))
+      throw Error("checkpoint_in: checkpoint " + std::to_string(c) + " that " + P + " names is missing " + CkptModel(base, N, r));
+  LoadShards(base + ".model");
+  for (int r = 0; r < N; ++r)
+    if (st->id_ranges[r] > 0) ShardEngine(r)->Check(dfb_id_range_set(ShardEngine(r)->handle(), st->id_ranges[r]), "dfb_id_range_set");
+  pos_.minibatches = st->minibatches;
+  ckpt_seq_ = static_cast<int>(c) + 1;
+  ckpt_prev_ = param_.checkpoint_out == P ? static_cast<int>(c) : -1;
+  if (verbose) printf("Resuming from checkpoint %lld of %s: epoch %d, minibatch %llu\n", c, P.c_str(), st->epoch,
+                      static_cast<unsigned long long>(st->minibatches));
+  resume_ = std::move(st);
 }
 
 }  // namespace difacto

@@ -164,6 +164,76 @@ static void BatchReader_StreamedChunks() {
   }
 }
 
+// the state record of a mid-epoch checkpoint reads back as it was written, float bits and all
+static void CheckpointState_RoundTrip() {
+  CheckpointState st;
+  st.settings = {{"data_in", "a b.libsvm"}, {"batch_size", "100"}, {"id_bits", ""}};
+  st.epoch = 3;
+  st.workers = {{2, 17}, {5, 0}};
+  st.has_rand = true;
+  for (size_t i = 0; i < RandState::kBytes; ++i) st.rand.bytes[i] = static_cast<unsigned char>(i * 7 + 1);
+  const float odd[5] = {1.0f / 3, -0.0f, 1e-38f, 123456.789f, 42.f};
+  for (int i = 0; i < 5; ++i) { st.epoch_prog[i] = odd[i]; st.part_prog[i] = odd[4 - i] * 3; }
+  st.pre_loss = 0.1f; st.pre_val_auc = 77.5f;
+  st.minibatches = (1ULL << 40) + 3;
+  st.id_ranges = {0, 37};
+  const std::string rec = st.Serialize();
+  const CheckpointState back = CheckpointState::Parse(rec);
+  EXPECT_TRUE(back.Serialize() == rec);
+  EXPECT_TRUE(back.settings == st.settings);
+  EXPECT_EQ(back.epoch, 3);
+  EXPECT_EQ(back.workers.size(), size_t(2));
+  EXPECT_EQ(back.workers[0].part, 2);
+  EXPECT_EQ(back.workers[0].consumed, uint64_t(17));
+  EXPECT_TRUE(memcmp(back.epoch_prog, st.epoch_prog, sizeof(st.epoch_prog)) == 0);
+  EXPECT_TRUE(memcmp(back.part_prog, st.part_prog, sizeof(st.part_prog)) == 0);
+  EXPECT_TRUE(memcmp(back.rand.bytes, st.rand.bytes, RandState::kBytes) == 0);
+  EXPECT_EQ(back.minibatches, st.minibatches);
+  EXPECT_TRUE(back.id_ranges == st.id_ranges);
+  // a different setting is refused by name; a truncated record is refused
+  bool named = false;
+  try {
+    back.CheckSettings({{"batch_size", "200"}});
+  } catch (const Error& e) {
+    named = std::string(e.what()).find("batch_size") != std::string::npos;
+  }
+  EXPECT_TRUE(named);
+  bool truncated = false;
+  try {
+    CheckpointState::Parse(rec.substr(0, rec.size() - 3));
+  } catch (const Error&) {
+    truncated = true;
+  }
+  EXPECT_TRUE(truncated);
+}
+
+// rand() saved before a reference-order reader starts and restored later gives that reader's batches again, whatever
+// was drawn in between
+static void CheckpointState_RandRestoresTheReader() {
+  auto dump = [](std::vector<std::vector<feaid_t>>* out) {
+    BatchReader r(DataPath(), "libsvm", 0, 1, 10, 30, 0.5f, 0, 0, ShuffleOrder::kReference);
+    while (r.Next()) {
+      auto b = r.Value();
+      out->push_back(std::vector<feaid_t>(b.index, b.index + b.offset[b.size]));
+      out->back().push_back(static_cast<feaid_t>(b.size));
+    }
+  };
+  const RandState at = RandState::Save();
+  std::vector<std::vector<feaid_t>> first, again, moved;
+  dump(&first);
+  dump(&moved);                // rand() has moved on: another order
+  at.Restore();
+  dump(&again);
+  EXPECT_TRUE(first.size() >= 3);
+  EXPECT_TRUE(first == again);
+  EXPECT_TRUE(first != moved);
+  for (int i = 0; i < 1000; ++i) rand();
+  at.Restore();
+  const int x = rand();
+  at.Restore();
+  EXPECT_EQ(rand(), x);
+}
+
 static void ArgParser_LastValueWins() {
   ArgParser p;
   p.AddArg("V_dim=64");
@@ -317,6 +387,8 @@ static const Case kCases[] = {
     {"BatchReader.Read", BatchReader_Read}, {"BatchReader.RandRead", BatchReader_RandRead},
     {"BatchReader.PartRead", BatchReader_PartRead},
     {"BatchReader.StreamedChunks", BatchReader_StreamedChunks},
+    {"CheckpointState.RoundTrip", CheckpointState_RoundTrip},
+    {"CheckpointState.RandRestoresTheReader", CheckpointState_RandRestoresTheReader},
     {"GpuFMLoss.NoV", GpuFMLoss_NoV}, {"GpuFMLoss.HasV", GpuFMLoss_HasV},
     {"GpuSGDLearner.Basic", GpuSGDLearner_Basic}, {"GpuSGDUpdater.SaveLoad", GpuSGDUpdater_SaveLoad},
     {"GpuSGDLearner.PluginCallsEqualFused", GpuSGDLearner_PluginCallsEqualFused}};

@@ -319,8 +319,40 @@ int dfb_restore_read(dfb_handle h, dfb_read_fn read_fn, void* ctx, uint32_t part
 int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes);
 int dfb_snapshot(dfb_handle h, int save_aux, void* buf, size_t bytes);
 int dfb_restore(dfb_handle h, const void* buf, size_t bytes, int* has_aux_out);
+/* checkpoint while training continues.  dfb_snapshot_begin waits for every stream of the handle, as
+ * dfb_snapshot_write does, copies the table's slots, its V rows and its counts and InitV state into fresh device
+ * memory, waits for the copy and returns: the handle is free to train from then on.  The copy takes the table's
+ * slots (32 bytes each) plus n_vrows V rows (dfb_row_stride floats each); when
+ * that memory cannot be had it returns DFB_ERR_CAPACITY and changes nothing.  The copy comes from the device's default
+ * memory pool and goes back to the device after its release.  On an engine that can still grow (table_capacity_max /
+ * V_capacity_max above the current capacities) begin also returns DFB_ERR_CAPACITY, changing nothing, when the free
+ * device memory would not cover the copy and that growth besides, so that a copy never takes the memory a later
+ * rehash or row-pool mapping needs.  At most one frozen snapshot per handle
+ * (a second begin is DFB_ERR_INVALID); it does not follow the handle's later growth (a rehash frees the old table,
+ * not the copy).
+ * dfb_frozen_write streams the copy through the same writer as dfb_snapshot_write, byte for byte what
+ * dfb_snapshot_write would have written at the moment of begin, on a low-priority stream of its own with its own
+ * device workspace, pinned chunks and error message (dfb_frozen_error).  It touches nothing of the handle, so it may
+ * run on another host thread while the handle's owning thread keeps enqueuing steps.  It may be called more than
+ * once; a write_fn error fails that call only.
+ * dfb_frozen_release frees the copy (stream-ordered after the writer's work); call it on the handle's owning thread
+ * once no dfb_frozen_write is running.  dfb_destroy releases a copy left behind. */
+typedef struct dfb_frozen_s* dfb_frozen;
+int dfb_snapshot_begin(dfb_handle h, int save_aux, dfb_frozen* out);
+int dfb_frozen_write(dfb_frozen f, size_t chunk_bytes, dfb_write_fn write_fn, void* ctx);
+const char* dfb_frozen_error(dfb_frozen f);
+int dfb_frozen_release(dfb_frozen f);
 /* state of the InitV random stream (SGDUpdaterParam::seed after the rand_r calls so far) */
 int dfb_rng_state(dfb_handle h, uint32_t* seed);
+/* the id range an engine with id_bits = 0 has learned from its raw batches (see id_bits), as a bit count: the ids
+ * seen so far lie below 2^bits (exactly: the byte-reversed keys have no bit set below 64 - bits).  get waits for the
+ * key masks still in flight and returns 0 when nothing has been learned yet; set gives an engine that has learned
+ * nothing that range (1 <= bits <= 64), and it then sorts, widens and drops batches exactly as the engine that
+ * learned it.  Together with a snapshot this is all the engine state a resumed run needs: the InitV state travels in
+ * the snapshot header, and the sharded store's per-step stamps (entry pad, in [1, 2^24)) never equal the 0 every
+ * restored entry carries. */
+int dfb_id_range_get(dfb_handle h, int* bits);
+int dfb_id_range_set(dfb_handle h, int bits);
 
 /* ---------------------------------------------------------------------------------
  * key-range sharding (multi-GPU).  ps-lite Postoffice::GetServerKeyRanges
