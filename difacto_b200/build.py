@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libdifacto_b200.so")
 SOURCES = ["kernels_fm.cu", "kernels_table.cu", "kernels_localize.cu", "kernels_shard.cu", "kernels_checkpoint.cu",
-           "engine.cu", "shard.cu", "checkpoint.cu", "growth.cu"]
+           "kernels_prune.cu", "engine.cu", "shard.cu", "checkpoint.cu", "growth.cu", "prune.cu"]
 HEADERS = ["dfb_internal.cuh", "dfb_device.cuh", "engine_internal.cuh", "shard_layout.cuh",
            os.path.join("..", "..", "include", "difacto_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")

@@ -18,6 +18,16 @@
 
 using namespace dfb;  // NOLINT
 
+// a checkpoint runs between steps: wait for everything enqueued on any of the handle's streams
+int dfbh::drain(dfb_engine* h) {
+  DFB_CUDA(h, cudaStreamSynchronize(h->copy_stream));
+  DFB_CUDA(h, cudaStreamSynchronize(h->loc_stream));
+  DFB_CUDA(h, cudaStreamSynchronize(h->aux_stream));
+  if (h->shard) DFB_TRY(dfbh::shard_sync(h));
+  DFB_CUDA(h, cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
 namespace {
 
 struct SnapHeader {
@@ -111,15 +121,7 @@ struct PinnedChunks {
   }
 };
 
-// a checkpoint runs between steps: wait for everything enqueued on any of the handle's streams
-int drain(dfb_engine* h) {
-  DFB_CUDA(h, cudaStreamSynchronize(h->copy_stream));
-  DFB_CUDA(h, cudaStreamSynchronize(h->loc_stream));
-  DFB_CUDA(h, cudaStreamSynchronize(h->aux_stream));
-  if (h->shard) DFB_TRY(dfbh::shard_sync(h));
-  DFB_CUDA(h, cudaStreamSynchronize(h->stream));
-  return 0;
-}
+using dfbh::drain;
 
 int read_state(dfb_engine* h, TableState* st) {
   DFB_CUDA(h, cudaMemcpyAsync(st, h->tab.state, sizeof(TableState), cudaMemcpyDeviceToHost, h->stream));

@@ -237,6 +237,8 @@ int launch_grad_finalize_dense(int V_dim, int ks, size_t nkeys, const int* hasv,
 int launch_table_init(Table& t, unsigned seed, cudaStream_t s);
 // empties new_t (new_t.cap >= old_t.cap slots) and re-inserts every entry of old_t into it, bytes unchanged
 int launch_table_rehash(const Table& old_t, const Table& new_t, cudaStream_t s);
+// inserts the n entries src[n] (distinct keys, none in t), all 32 bytes as they are, into t: k_table_rehash's insert
+int launch_table_insert(const Entry* src, uint64_t n, const Table& t, cudaStream_t s);
 // find (or insert) keys; slot_out[i] = hash position or -1.  When pull outputs are non-null also
 // emits w and vrow of each entry.
 // n is a host count, or (dn != nullptr) the capacity with the actual count read from the device
@@ -314,6 +316,16 @@ int launch_rst_chunk(Table& t, const unsigned* buf, const unsigned* roff, size_t
                      unsigned nparts, unsigned shard, unsigned nshards, unsigned long long* flags,
                      unsigned long long* rank, void* tmp, size_t tmp_bytes, cudaStream_t s);
 int launch_rst_seed(Table& t, unsigned seed, cudaStream_t s);
+
+// ---- dfb_prune (kernels_prune.cu, host side in prune.cu) ----
+// an entry is dropped when w == 0, it has no V row and fea_cnt <= max_count.  Both launches run prune_grid(t.cap)
+// blocks.  count: tot[2] = {kept, dropped} and blk_kept[grid] (zeroed by the caller).  rebuild: the kept entries into
+// kept[n_kept] (n_kept = tot[0]), the slots emptied, the kept entries re-inserted, n_keys lowered by tot[1].
+int prune_grid(uint64_t cap);
+int launch_prune_count(const Table& t, float max_count, int grid, unsigned long long* tot, unsigned* blk_kept,
+                       cudaStream_t s);
+int launch_prune_rebuild(Table& t, float max_count, int grid, const unsigned long long* tot, const unsigned* blk_kept,
+                         Entry* kept, uint64_t n_kept, cudaStream_t s);
 
 // ---- GPU localizer (kernels_localize.cu): Localizer::Compact + the CSC view from one radix sort ----
 size_t localize_sort_tmp_bytes(size_t nnz);

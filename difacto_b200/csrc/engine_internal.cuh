@@ -200,7 +200,12 @@ int reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows);
 // cap, mask, ks and rs, has vcap = n_vrows and no state or progress: the snapshot writer's view of a table.
 int table_copy(dfb_engine* h, uint64_t n_vrows, dfb::Table* out);
 void table_copy_free(dfb::Table* t, cudaStream_t s);   // stream-ordered on s
+// after a dfb_prune (which waited for every stream): the table holds exactly n_keys keys and n_vrows V rows, and no
+// inserting call is in flight
+void counts_known(dfb_engine* h, uint64_t n_keys, uint64_t n_vrows);
 void frozen_destroy(dfb_frozen_s* f);   // checkpoint.cu: frees the copy after its stream's work
+int drain(dfb_engine* h);               // checkpoint.cu: wait for everything enqueued on any of the handle's streams
 void shard_destroy(dfb_engine* h);      // shard.cu
 int shard_sync(dfb_engine* h);          // shard.cu: drain the shard's streams
+bool shard_step_open(const dfb_engine* h);   // shard.cu: a sharded step is begun and its phase 4 not yet enqueued
 }  // namespace dfbh

@@ -226,6 +226,13 @@ int dfbh::reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows) {
   return 0;
 }
 
+void dfbh::counts_known(dfb_engine* h, uint64_t n_keys, uint64_t n_vrows) {
+  dfb_engine::Growth& g = h->grow;
+  g.head = g.seq;                       // the copies in flight are complete, and older than these counts
+  g.known_k = n_keys; g.known_v = n_vrows;
+  g.known_at_k = g.total_k; g.known_at_v = g.total_v;
+}
+
 int dfbh::table_copy(dfb_engine* h, uint64_t n_vrows, Table* out) {
   const Table& t = h->tab;
   Table c = t;

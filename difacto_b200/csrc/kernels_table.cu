@@ -1201,6 +1201,12 @@ int launch_table_rehash(const Table& old_t, const Table& new_t, cudaStream_t s) 
   return 2;
 }
 
+int launch_table_insert(const Entry* src, uint64_t n, const Table& t, cudaStream_t s) {
+  if (n == 0) return 0;
+  k_table_rehash<<<grid_for(n, 256, num_sms() * 8), 256, 0, s>>>(src, n, t.tab, t.mask, 1);
+  return 1;
+}
+
 int launch_lookup(Table& t, const uint64_t* keys, size_t n, const unsigned long long* dn, bool insert,
                   int* slot_out, float* w_out, int* vrow_out, int2* wv_out, cudaStream_t s) {
   if (n == 0) return 0;

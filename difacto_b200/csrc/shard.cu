@@ -425,6 +425,8 @@ int dfbh::shard_sync(dfb_engine* h) {
   return DFB_OK;
 }
 
+bool dfbh::shard_step_open(const dfb_engine* h) { return h->shard && h->shard->cx.open; }
+
 extern "C" {
 
 int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t max_nnz, size_t seg_keys,

@@ -14,6 +14,7 @@ LINK = ["-L", LIBDIR, "-ldifacto_b200", f"-Wl,-rpath,{LIBDIR}", "-Wl,-rpath,$ORI
 TARGETS = {
     "difacto_b200": ["src/main.cc", "src/sgd_learner.cc"],
     "host_tests": ["tests/host_tests.cc", "src/sgd_learner.cc"],
+    "prune_settings_tests": ["tests/prune_settings_tests.cc", "src/sgd_learner.cc"],
     "batch_dump": ["tests/batch_dump.cc"],
 }
 

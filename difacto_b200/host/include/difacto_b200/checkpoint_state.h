@@ -116,11 +116,14 @@ struct CheckpointState {
     if (p != s.size()) throw Error("checkpoint state corrupt (trailing bytes)");
     return st;
   }
-  /** throws naming the first setting that differs from `now` */
-  void CheckSettings(const std::vector<std::pair<std::string, std::string>>& now) const {
+  /** throws naming the first setting that differs from `now`.  `later`: settings the record format gained after
+   * checkpoints were first written, with the value a record that lacks one stands for (the setting's default) */
+  void CheckSettings(const std::vector<std::pair<std::string, std::string>>& now,
+                     const std::vector<std::pair<std::string, std::string>>& later = {}) const {
     for (const auto& kv : now) {
       const std::string* saved = nullptr;
       for (const auto& s : settings) if (s.first == kv.first) saved = &s.second;
+      if (!saved) for (const auto& s : later) if (s.first == kv.first) saved = &s.second;
       if (!saved) throw Error("checkpoint_in: the checkpoint does not record " + kv.first);
       if (*saved != kv.second)
         throw Error("checkpoint_in: " + kv.first + " differs from the checkpoint's (" + kv.first + " = " + *saved +

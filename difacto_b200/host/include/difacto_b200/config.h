@@ -94,6 +94,10 @@ struct SGDLearnerParam {
   // checkpoint_out.<c>.* and the pointer file checkpoint_out; checkpoint_in resumes the run a pointer file names
   std::string checkpoint_out, checkpoint_in;
   long long checkpoint_period = 0;
+  // engine-only: every prune_period training minibatches per worker (0: never) drop the table entries with w == 0, no
+  // V row and fea_cnt <= prune_count (dfb_prune)
+  long long prune_period = 0;
+  float prune_count = 0;
 
   KWArgs InitAllowUnknown(const KWArgs& kwargs) {
     KWArgs remain;
@@ -121,6 +125,8 @@ struct SGDLearnerParam {
         else if (k == "checkpoint_out") checkpoint_out = v;
         else if (k == "checkpoint_in") checkpoint_in = v;
         else if (k == "checkpoint_period") checkpoint_period = std::stoll(v);
+        else if (k == "prune_period") prune_period = std::stoll(v);
+        else if (k == "prune_count") prune_count = std::stof(v);
         else remain.push_back(kv);
       } catch (const std::logic_error&) {
         throw ParamError("Invalid Parameter format for " + k + " value='" + v + "'");
@@ -130,6 +136,8 @@ struct SGDLearnerParam {
     if (batch_size < 0) throw ParamError("Required parameter batch_size of int is not presented");   // sgd_param.h:58
     if (checkpoint_period < 0) throw ParamError("checkpoint_period must be >= 0");
     if (checkpoint_period > 0 && checkpoint_out.empty()) throw ParamError("checkpoint_period needs checkpoint_out");
+    if (prune_period < 0) throw ParamError("prune_period must be >= 0");
+    if (prune_count != prune_count) throw ParamError("prune_count must be a number");
     return remain;
   }
 };

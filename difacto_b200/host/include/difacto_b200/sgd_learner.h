@@ -65,6 +65,14 @@ class SGDLearner : public Learner {
   sgd::Progress Predict();
   /** set false to silence the per-epoch log lines */
   bool verbose = true;
+  /** the settings that fix the minibatches and the model, as parsed values (the engine's defaults for the keys not
+   * given): a checkpoint resumes only under the same settings */
+  static std::vector<std::pair<std::string, std::string>> Settings(const SGDLearnerParam& p, const KWArgs& kwargs);
+  /** the settings a checkpoint written before they existed does not record, with the value it ran under: the
+   * default, so such a checkpoint resumes under the defaults and is refused under anything else */
+  static std::vector<std::pair<std::string, std::string>> SettingsAddedLater() {
+    return {{"prune_period", "0"}, {"prune_count", "0"}};
+  }
 
  protected:
   void RunScheduler() override;
@@ -80,8 +88,13 @@ class SGDLearner : public Learner {
   void LoadShards(const std::string& base);
   /** checkpoint_in: the model, the id ranges and the position in the run of the checkpoint the pointer file names */
   void LoadCheckpoint();
-  /** after a training minibatch per worker: a checkpoint when the period has come round.  The model is frozen on
-   * every GPU now; a helper thread writes it, then the state record, then renames the pointer file */
+  /** after a training minibatch per worker (every rank's step collected): counts it, then prunes and checkpoints
+   * when their periods have come round, the prune first */
+  void EndMinibatch();
+  /** prune_period: every rank drops its entries with w == 0, no V row and fea_cnt <= prune_count (dfb_prune) */
+  void MaybePrune();
+  /** a checkpoint when the period has come round.  The model is frozen on every GPU now; a helper thread writes it,
+   * then the state record, then renames the pointer file */
   void MaybeCheckpoint();
   /** waits for the checkpoint write in flight and releases its device copies; throws what it failed with */
   void WaitCheckpoint();

@@ -59,15 +59,13 @@ SGDLearner::~SGDLearner() {
   delete store_;
 }
 
-// SGDLearner::Init, sgd_learner.cc:229-246
-KWArgs SGDLearner::Init(const KWArgs& kwargs) {
-  KWArgs remain = param_.InitAllowUnknown(kwargs);
-  // what fixes the minibatches and the model: a checkpoint resumes only under the same settings
-  settings_ = {{"data_in", param_.data_in}, {"data_val", param_.data_val}, {"data_format", param_.data_format},
-               {"loss", param_.loss}, {"num_gpus", std::to_string(param_.num_gpus)},
-               {"num_jobs_per_epoch", std::to_string(param_.num_jobs_per_epoch)},
-               {"batch_size", std::to_string(param_.batch_size)}, {"shuffle", std::to_string(param_.shuffle)},
-               {"neg_sampling", FloatSetting(param_.neg_sampling)}};
+std::vector<std::pair<std::string, std::string>> SGDLearner::Settings(const SGDLearnerParam& p, const KWArgs& kwargs) {
+  std::vector<std::pair<std::string, std::string>> s = {
+      {"data_in", p.data_in}, {"data_val", p.data_val}, {"data_format", p.data_format}, {"loss", p.loss},
+      {"num_gpus", std::to_string(p.num_gpus)}, {"num_jobs_per_epoch", std::to_string(p.num_jobs_per_epoch)},
+      {"batch_size", std::to_string(p.batch_size)}, {"shuffle", std::to_string(p.shuffle)},
+      {"neg_sampling", FloatSetting(p.neg_sampling)}, {"prune_period", std::to_string(p.prune_period)},
+      {"prune_count", FloatSetting(p.prune_count)}};
   // SGDUpdaterParam (sgd_param.h:94-106) and id_bits, with the engine's defaults for the keys not given
   struct Key { const char* name; const char* dflt; bool is_float; };
   const Key keys[] = {{"l1", "1", true}, {"l2", "0", true}, {"V_l2", ".01", true}, {"lr", ".01", true},
@@ -77,8 +75,15 @@ KWArgs SGDLearner::Init(const KWArgs& kwargs) {
   for (const Key& k : keys) {
     std::string v = k.dflt;
     for (const auto& kv : kwargs) if (kv.first == k.name) v = kv.second;
-    settings_.push_back(std::make_pair(std::string(k.name), k.is_float ? FloatSetting(v) : IntSetting(v)));
+    s.push_back(std::make_pair(std::string(k.name), k.is_float ? FloatSetting(v) : IntSetting(v)));
   }
+  return s;
+}
+
+// SGDLearner::Init, sgd_learner.cc:229-246
+KWArgs SGDLearner::Init(const KWArgs& kwargs) {
+  KWArgs remain = param_.InitAllowUnknown(kwargs);
+  settings_ = Settings(param_, kwargs);
   auto* updater = new GpuSGDUpdater();
   std::shared_ptr<Updater> holder(updater);
   remain = updater->Init(remain);
@@ -462,7 +467,7 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
       for (int r = 0; r < N; ++r) { pos_.workers[r].part = w[r].part; pos_.workers[r].consumed = w[r].consumed; }
       epoch_prog_ = prog;
       part_prog_ = nullptr;
-      MaybeCheckpoint();
+      EndMinibatch();
       epoch_prog_ = nullptr;
     }
   }
@@ -616,7 +621,7 @@ void SGDLearner::IterateData(const sgd::Job& job, sgd::Progress* progress) {
     }
     if (train) {
       ++pos_.workers[0].consumed;
-      MaybeCheckpoint();
+      EndMinibatch();
     }
   }
 }
@@ -682,8 +687,35 @@ void RemoveCheckpoint(const std::string& P, int c, int N) {
 
 // checkpoint c: P.<c>.model (P.<c>.model_part-<r>), P.<c>.state, then P names c.  Until the rename, P names c - 1,
 // which stays complete on the disk; it is removed after.
-void SGDLearner::MaybeCheckpoint() {
+void SGDLearner::EndMinibatch() {
   ++pos_.minibatches;
+  MaybePrune();
+  MaybeCheckpoint();
+}
+
+// every rank's table at the same boundary, after all ranks' steps: the prune waits for each engine's streams
+void SGDLearner::MaybePrune() {
+  if (param_.prune_period <= 0 || pos_.minibatches % static_cast<uint64_t>(param_.prune_period) != 0) return;
+  uint64_t dropped = 0, n_keys = 0;
+  for (int r = 0; r < param_.num_gpus; ++r) {
+    const auto& e = ShardEngine(r);
+    uint64_t d = 0, k = 0;
+    int rc = dfb_prune(e->handle(), param_.prune_count, &d);
+    if (rc == DFB_ERR_CAPACITY && !frozen_.empty()) {    // no room for the workspace beside a checkpoint's device copy
+      WaitCheckpoint();
+      rc = dfb_prune(e->handle(), param_.prune_count, &d);
+    }
+    e->Check(rc, "dfb_prune");
+    e->Check(dfb_table_stats(e->handle(), &k, nullptr, nullptr, nullptr), "dfb_table_stats");
+    dropped += d;
+    n_keys += k;
+  }
+  if (verbose)
+    printf("Prune: minibatch %llu, dropped %llu, n_keys %llu\n", static_cast<unsigned long long>(pos_.minibatches),
+           static_cast<unsigned long long>(dropped), static_cast<unsigned long long>(n_keys));
+}
+
+void SGDLearner::MaybeCheckpoint() {
   if (param_.checkpoint_period <= 0 || pos_.minibatches % static_cast<uint64_t>(param_.checkpoint_period) != 0) return;
   WaitCheckpoint();
   const int N = param_.num_gpus;
@@ -764,7 +796,7 @@ void SGDLearner::LoadCheckpoint() {
   std::stringstream ss;
   ss << fs.rdbuf();
   std::unique_ptr<CheckpointState> st(new CheckpointState(CheckpointState::Parse(ss.str())));
-  st->CheckSettings(settings_);
+  st->CheckSettings(settings_, SettingsAddedLater());
   const int N = param_.num_gpus;
   if (static_cast<int>(st->workers.size()) != N || static_cast<int>(st->id_ranges.size()) != N)
     throw Error("checkpoint_in: " + base + ".state does not hold " + std::to_string(N) + " workers");

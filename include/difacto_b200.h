@@ -353,6 +353,16 @@ int dfb_rng_state(dfb_handle h, uint32_t* seed);
  * restored entry carries. */
 int dfb_id_range_get(dfb_handle h, int* bits);
 int dfb_id_range_set(dfb_handle h, int bits);
+/* Drops every entry with w == 0, no V row and fea_cnt <= max_count; returns how many entries it dropped.
+ * Such an entry adds nothing to any prediction: the forward reads a key the table lacks exactly so (w = 0, no V row).
+ * Predictions are therefore unchanged; a dropped key that comes back starts its FTRL state (fea_cnt, sqrt_g, z) from
+ * zero.  Entries with a V row are never dropped: V rows, n_vrows and the InitV state do not change, and every kept
+ * entry keeps its 32 bytes (its pad too).  n_keys drops by *n_dropped; the capacities stay, and the freed slots take
+ * new keys.  Like dfb_snapshot_begin it waits for every stream of the handle and runs between steps: during a sharded
+ * step (dfb_shard_begin_* .. dfb_shard_phase(4)) it is DFB_ERR_INVALID.  A frozen snapshot is a copy and is not
+ * changed.  The table is rebuilt in place with a workspace of 32 bytes per kept entry, taken before the table is
+ * touched: DFB_ERR_CAPACITY when it cannot be had, and then nothing has changed. */
+int dfb_prune(dfb_handle h, float max_count, uint64_t* n_dropped);
 
 /* ---------------------------------------------------------------------------------
  * key-range sharding (multi-GPU).  ps-lite Postoffice::GetServerKeyRanges
