@@ -40,6 +40,7 @@ EXPORTS = [
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
     "dfb_predict_raw_async", "dfb_predict_raw_dev", "dfb_shard_predict_async", "dfb_shard_begin_predict_async",
+    "dfb_row_bytes",
 ]
 
 _LIB = None
@@ -67,6 +68,7 @@ def lib():
         L.dfb_launch_count.restype = u64
         L.dfb_launch_count.argtypes = [vp]
         L.dfb_table_stats.argtypes = [vp] + [C.POINTER(u64)] * 4
+        L.dfb_row_bytes.argtypes = [vp] + [C.POINTER(u64)] * 2
         L.dfb_host_alloc.argtypes = [C.POINTER(vp), sz]
         L.dfb_host_free.argtypes = [vp]
         L.dfb_push_feacnt.argtypes = [vp, vp, sz, vp]
@@ -210,12 +212,13 @@ class Engine:
 
     The keyword arguments are dfb_create's keys (include/difacto_b200.h).  table_capacity / V_capacity are the initial
     capacities; with table_capacity_max / V_capacity_max above them the table and the V-row pool grow on demand, and
-    table_stats() reports the current capacities."""
+    table_stats() reports the current capacities.  score_only=True (optionally V_storage="bf16") makes a scoring-only
+    engine: restore and predict_raw* only, V rows without their AdaGrad halves; what it refuses raises DfbError."""
 
     def __init__(self, **kwargs):
         L = lib()
         ks = [str(k).encode() for k in kwargs]
-        vs = [str(v).encode() for v in kwargs.values()]
+        vs = [str(int(v) if isinstance(v, bool) else v).encode() for v in kwargs.values()]
         n = len(ks)
         ka = (C.c_char_p * n)(*ks)
         va = (C.c_char_p * n)(*vs)
@@ -260,6 +263,12 @@ class Engine:
         a, b, c, d = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_uint64()
         self._ck(self.L.dfb_table_stats(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return dict(n_keys=a.value, n_vrows=b.value, capacity=c.value, v_capacity=d.value)
+
+    def row_bytes(self):
+        """(bytes one V row takes in the row pool, n_vrows times that)"""
+        a, b = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.dfb_row_bytes(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
 
     def rng_state(self):
         s = C.c_uint32()

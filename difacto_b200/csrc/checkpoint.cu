@@ -347,6 +347,7 @@ int restore_read(dfb_engine* h, dfb_read_fn fn, void* ctx, uint32_t part, uint32
     default: return h->fail(DFB_ERR_INVALID, "device-side error " + std::to_string(h->h_prog->err) + " while restoring");
   }
   h->has_aux = first ? (wk.aux ? 1 : 0) : (h->has_aux && wk.aux ? 1 : 0);
+  if (h->score_only) h->has_aux = 0;    // V-only rows: the streams' aux data, if any, was not kept
   h->restored_parts++;
   if (has_aux_out) *has_aux_out = h->has_aux;
   return 0;
@@ -360,7 +361,7 @@ int clear_table(dfb_engine* h, int rc) {
   h->launches += launch_table_init(h->tab, h->prm.seed, h->stream);
   const cudaError_t e = cudaStreamSynchronize(h->stream);
   h->restored_parts = 0;
-  h->has_aux = 1;
+  h->has_aux = h->score_only ? 0 : 1;
   h->err = msg + "; the table was cleared";
   if (e != cudaSuccess) h->err += std::string(" (clearing failed: ") + cudaGetErrorString(e) + ")";
   return rc;
@@ -418,6 +419,7 @@ extern "C" {
 
 int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes) {
   if (!h || !bytes) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_snapshot_size");
   DFB_CUDA(h, cudaSetDevice(h->device));
   DFB_TRY(drain(h));
   TableState st;
@@ -429,6 +431,7 @@ int dfb_snapshot_size(dfb_handle h, int save_aux, size_t* bytes) {
 
 int dfb_snapshot_write(dfb_handle h, int save_aux, size_t chunk_bytes, dfb_write_fn fn, void* ctx) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_snapshot_write");
   if (!fn) return h->fail(DFB_ERR_INVALID, "write callback is NULL");
   ErrSink es{&h->err};
   DFB_TRY(check_chunk(&chunk_bytes, &es));
@@ -444,6 +447,7 @@ int dfb_snapshot_write(dfb_handle h, int save_aux, size_t chunk_bytes, dfb_write
 
 int dfb_snapshot_begin(dfb_handle h, int save_aux, dfb_frozen* out) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_snapshot_begin");
   if (!out) return h->fail(DFB_ERR_INVALID, "out is NULL");
   *out = nullptr;
   if (h->frozen) return h->fail(DFB_ERR_INVALID, "the handle already has a frozen snapshot (release it first)");
@@ -503,6 +507,7 @@ int dfb_restore_read(dfb_handle h, dfb_read_fn fn, void* ctx, uint32_t part, uin
 
 int dfb_snapshot(dfb_handle h, int save_aux, void* buf, size_t bytes) {
   if (!h || !buf) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_snapshot");
   size_t need = 0;
   DFB_TRY(dfb_snapshot_size(h, save_aux, &need));
   if (bytes < need) return h->fail(DFB_ERR_INVALID, "snapshot buffer too small");

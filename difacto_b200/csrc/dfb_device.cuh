@@ -59,6 +59,13 @@ __device__ __forceinline__ float4 ldg128_pol(const float* p, uint64_t pol) {
                : "l"(p), "l"(pol));
   return r;
 }
+// 4 bf16 columns of a scoring-only engine's V row (one 8-byte load), widened to fp32: exact, a 16-bit shift
+__device__ __forceinline__ float4 ldg_bf16x4_pol(const void* p, uint64_t pol) {
+  unsigned lo, hi;
+  asm volatile("ld.global.nc.L2::cache_hint.v2.b32 {%0, %1}, [%2], %3;" : "=r"(lo), "=r"(hi) : "l"(p), "l"(pol));
+  return make_float4(__uint_as_float(lo << 16), __uint_as_float(lo & 0xffff0000u),
+                     __uint_as_float(hi << 16), __uint_as_float(hi & 0xffff0000u));
+}
 __device__ __forceinline__ int2 ldg64_pol(const int2* p, uint64_t pol) {
   int2 r;
   asm volatile("ld.global.nc.L2::cache_hint.v2.s32 {%0, %1}, [%2], %3;" : "=r"(r.x), "=r"(r.y) : "l"(p), "l"(pol));

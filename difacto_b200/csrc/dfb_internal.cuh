@@ -8,6 +8,8 @@
 //                         ks = V_dim rounded up to 4 floats -- the reference's `new real_t[2n]`
 //                         (sgd_updater.cc:142).  The gather reads the first half (one contiguous
 //                         4k-byte chunk); the update reads and writes the whole 8k-byte row.
+//                         A scoring-only engine (score_only = 1) holds V only: VV[vcap][ks] of fp32 or bf16 elements
+//                         (Table::rs == ks, Table::vonly), and nothing that trains or saves runs on it.
 // V rows are allocated lazily from a bump pool, exactly when the reference calls InitV.
 #pragma once
 #include <cuda_runtime.h>
@@ -60,7 +62,9 @@ struct Table {
   float* Vcg = nullptr;
   uint64_t vcap = 0;
   int ks = 0;  // V_dim rounded up to a multiple of 4 floats
-  int rs = 0;  // stride between table rows in floats (2*ks); Vcg == V + ks
+  int rs = 0;  // stride between table rows in elements: 2*ks floats, Vcg == V + ks; a scoring-only engine: ks, no Vcg
+  int vonly = 0;   // a scoring-only engine's rows: 1 = fp32 V, 2 = bf16 V (V then points at 2-byte elements; only the
+                   // restore's scoring insert and the bf16 raw forward touch them).  0: the training layout
   TableState* state = nullptr;
   DevProgress* prog = nullptr;
 };
@@ -223,8 +227,10 @@ size_t l2_bytes();
 // returns number of kernel launches performed, or <0 on invalid configuration
 int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s);
 // predict only, on raw ids (b.ids): the specialised kernels probe the table (v.tab) for each nonzero's key instead of
-// reading a pulled view; v.vbase / vstride = the table rows.  -1 when V_dim has no specialised kernels
-int launch_fm_raw(const FmBatch& b, const FmView& v, cudaStream_t s);
+// reading a pulled view; v.vbase / vstride = the table rows.  -1 when V_dim has no specialised kernels.
+// bf16_rows (predict only; a scoring-only engine with V_storage = bf16): v.vbase points at bf16 elements and vstride
+// counts them; each lane widens its 4 columns to fp32 and everything after the load is the fp32 kernels' code
+int launch_fm_raw(const FmBatch& b, const FmView& v, bool bf16_rows, cudaStream_t s);
 // MODE 3: partial interaction sums of every source's rows (see PartArgs); v.vbase/vstride = the table rows
 int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s);
 int launch_grad_finalize(int V_dim, size_t nkeys, const float* weights, const int* V_pos,
@@ -311,7 +317,8 @@ size_t ckpt_sort_tmp_bytes(size_t n);
 int launch_ckpt_pass(const Table& t, unsigned b0, unsigned b1, size_t n, int aux, int k, const CkptWs& ws,
                      cudaStream_t s);
 size_t rst_scan_tmp_bytes(size_t n);
-// n records of a chunk (roff: word offset of each record in buf): keep this shard's keys and insert them
+// n records of a chunk (roff: word offset of each record in buf): keep this shard's keys and insert them.  A table of
+// V-only rows (t.vonly) gets V alone, rounded to nearest even when the rows are bf16; the records' cg is skipped
 int launch_rst_chunk(Table& t, const unsigned* buf, const unsigned* roff, size_t n, int aux, int k, unsigned part,
                      unsigned nparts, unsigned shard, unsigned nshards, unsigned long long* flags,
                      unsigned long long* rank, void* tmp, size_t tmp_bytes, cudaStream_t s);

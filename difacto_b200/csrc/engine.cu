@@ -319,7 +319,7 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   }
   if (nrows) {
     StageTimer tm(h, 1);
-    const int nl = probe ? launch_fm_raw(b, v, s) : launch_fm(b, v, h->force_generic, s);
+    const int nl = probe ? launch_fm_raw(b, v, false, s) : launch_fm(b, v, h->force_generic, s);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
     h->launches += nl;
   }
@@ -599,7 +599,7 @@ int predict_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, 
   }
   if (nrows) {
     StageTimer tm(h, 1);
-    const int nl = launch_fm_raw(b, v, s);
+    const int nl = launch_fm_raw(b, v, h->tab.vonly == 2, s);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
     h->launches += nl;
   }
@@ -643,6 +643,7 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   p.l1 = 1.f; p.l2 = 0.f; p.V_l2 = .01f; p.lr = .01f; p.lr_beta = 1.f; p.V_lr = .01f; p.V_lr_beta = 1.f;
   p.V_init_scale = .01f; p.V_threshold = 10; p.V_dim = -1; p.seed = 0;
   long long table_capacity = 1 << 20, v_capacity = -1, table_capacity_max = -1, v_capacity_max = -1;
+  bool v_bf16 = false;
   struct FR { const char* name; float* dst; float lo, hi; };
   FR fr[] = {{"l1", &p.l1, 0, 1e10f}, {"l2", &p.l2, 0, 1e10f}, {"V_l2", &p.V_l2, 0, 1e10f},
              {"lr", &p.lr, 0, 10}, {"lr_beta", &p.lr_beta, 0, 1e10f}, {"V_lr", &p.V_lr, 0, 1e10f},
@@ -687,6 +688,12 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else if (k == "l2_hints") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->l2_hints = (int)x; }
     else if (k == "id_bits") { if (!need_int(0, 64)) { delete h; return DFB_ERR_PARAM; } h->id_bits = (int)x; }
     else if (k == "shard_timeout_ms") { if (!need_int(1, 3600000)) { delete h; return DFB_ERR_PARAM; } h->shard_timeout_ms = x; }
+    else if (k == "score_only") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->score_only = (int)x; }
+    else if (k == "V_storage") {
+      if (v == "fp32") v_bf16 = false;
+      else if (v == "bf16") v_bf16 = true;
+      else return bad("V_storage must be 'fp32' or 'bf16'");
+    }
     else if (k == "scatter") {
       if (v == "sorted") h->scatter_sorted = 1;
       else if (v == "atomic") h->scatter_sorted = 0;
@@ -695,6 +702,11 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else h->unknown.push_back(std::make_pair(k, v));
   }
   if (p.V_dim < 0) return bad("Required parameter V_dim of int is not presented");   // sgd_param.h:104
+  if (v_bf16 && !h->score_only) return bad("V_storage = bf16 needs score_only = 1 (training on 2-byte rows is not offered)");
+  // a scoring-only engine predicts with the raw-id forward alone: the other widths' predict step is the validation
+  // step, which reads a pulled view the engine does not build
+  if (h->score_only && (h->force_generic || !fm_fast_supported(p.V_dim)))
+    return bad("score_only = 1 needs 0 <= V_dim <= 128 and force_generic = 0");
   // the initial capacities and the maxima they may grow to (equal by default: nothing grows)
   if (table_capacity_max < 0) table_capacity_max = table_capacity;
   if (table_capacity_max < table_capacity) return bad("table_capacity_max must be >= table_capacity");
@@ -741,7 +753,9 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
   t.mask = t.cap - 1;
   t.ks = (p.V_dim + 3) / 4 * 4;
   t.vcap = (uint64_t)v_capacity;
-  t.rs = 2 * t.ks;
+  t.rs = h->score_only ? t.ks : 2 * t.ks;
+  t.vonly = h->score_only ? (v_bf16 ? 2 : 1) : 0;
+  if (h->score_only) h->has_aux = 0;
   if (const int rc = dfbh::capacity_create(h)) {
     g_create_error = h->err;
     cudaGetLastError();
@@ -830,6 +844,16 @@ uint64_t dfb_launch_count(dfb_handle h) { return h ? h->launches : 0; }
 void* dfb_stream(dfb_handle h) { return h ? (void*)h->stream : nullptr; }
 int dfb_row_stride(dfb_handle h) { return h ? h->tab.ks : 0; }
 
+int dfb_row_bytes(dfb_handle h, uint64_t* bytes_per_row, uint64_t* bytes_in_use) {
+  if (!h) return DFB_ERR_INVALID;
+  const uint64_t rb = (uint64_t)h->tab.rs * (h->tab.vonly == 2 ? 2 : 4);
+  uint64_t n_vrows = 0;
+  DFB_TRY(dfb_table_stats(h, nullptr, &n_vrows, nullptr, nullptr));
+  if (bytes_per_row) *bytes_per_row = rb;
+  if (bytes_in_use) *bytes_in_use = n_vrows * rb;
+  return DFB_OK;
+}
+
 int dfb_table_stats(dfb_handle h, uint64_t* n_keys, uint64_t* n_vrows, uint64_t* capacity, uint64_t* v_capacity) {
   if (!h) return DFB_ERR_INVALID;
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -888,6 +912,7 @@ int dfb_host_free(void* ptr) { return cudaFreeHost(ptr) == cudaSuccess ? DFB_OK 
 // ------------------------------------------------------------------------------------------
 int dfb_push_feacnt(dfb_handle h, const uint64_t* keys, size_t n, const float* cnt) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_push_feacnt");
   if (n && (!keys || !cnt)) return h->fail(DFB_ERR_INVALID, "keys/cnt is NULL");
   if (n > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "too many keys");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -905,6 +930,7 @@ int dfb_push_feacnt(dfb_handle h, const uint64_t* keys, size_t n, const float* c
 int dfb_pull(dfb_handle h, const uint64_t* keys, size_t n, float* vals_out, size_t vals_cap, int* lens_out,
              size_t* nvals, size_t* nlens) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_pull");
   if (!nvals || !nlens) return h->fail(DFB_ERR_INVALID, "nvals/nlens is NULL");
   if (n && (!keys || !vals_out)) return h->fail(DFB_ERR_INVALID, "keys/vals_out is NULL");
   if (n > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "too many keys");
@@ -949,6 +975,7 @@ int dfb_pull(dfb_handle h, const uint64_t* keys, size_t n, float* vals_out, size
 int dfb_push_grad(dfb_handle h, const uint64_t* keys, size_t n, const float* grads, size_t nvals,
                   const int* lens, size_t nlens) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_push_grad");
   if (n && (!keys || !grads)) return h->fail(DFB_ERR_INVALID, "keys/grads is NULL");
   if (n > 0x7fffffffULL) return h->fail(DFB_ERR_INVALID, "too many keys");
   if (!h->has_aux) return h->fail(DFB_ERR_INVALID, "no aux data");   // CHECK(has_aux_), sgd_updater.cc:75
@@ -1010,6 +1037,7 @@ int dfb_predict(dfb_handle h, size_t nrows, const uint64_t* offset, const uint32
                 const float* weights, size_t nweights, const int* w_pos, const int* V_pos, size_t npos,
                 float* pred) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_predict");
   if (nrows == 0) return DFB_OK;
   if (!pred) return h->fail(DFB_ERR_INVALID, "pred is NULL");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -1038,6 +1066,7 @@ int dfb_calc_grad(dfb_handle h, size_t nrows, const uint64_t* offset, const uint
                   const float* label, const float* weights, size_t nweights, const int* w_pos, const int* V_pos,
                   size_t npos, const float* pred, float* grad) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_calc_grad");
   if (nrows == 0) return DFB_OK;
   if (!pred || !grad || !label) return h->fail(DFB_ERR_INVALID, "pred/grad/label is NULL");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -1119,6 +1148,7 @@ int dfb_train_step_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d
                        const float* d_value_or_null, const float* d_label, const uint64_t* d_keys, size_t nkeys,
                        const float* d_cnt_or_null, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_train_step_dev");
   DFB_CUDA(h, cudaSetDevice(h->device));
   return step_dev(h, nrows, nnz, d_offset, d_index, d_value_or_null, d_label, d_keys, nkeys, d_cnt_or_null,
                   is_train);
@@ -1155,6 +1185,7 @@ int dfb_train_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, con
                          const float* value, const float* label, const uint64_t* keys, size_t nkeys,
                          const float* cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_train_step_async");
   DFB_TRY(check_csr(h, nrows, offset));
   if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
   if (nkeys && !keys) return h->fail(DFB_ERR_INVALID, "keys is NULL");
@@ -1296,6 +1327,7 @@ int dfb_localize(dfb_handle h, size_t nrows, const uint64_t* offset, const uint6
 int dfb_train_step_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
                            const float* d_value_or_null, const float* d_label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_train_step_raw_dev");
   DFB_CUDA(h, cudaSetDevice(h->device));
   return step_raw_dev(h, nrows, nnz, d_offset, d_ids, d_value_or_null, d_label, push_cnt, is_train, nullptr);
 }
@@ -1333,6 +1365,7 @@ int dfb_prefetch_raw(dfb_handle h, size_t nrows, const uint64_t* offset, const u
 static int raw_async_impl(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
                           const float* value, const float* label, int push_cnt, int is_train, bool exact_range) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_train_step_raw");
   DFB_TRY(check_csr(h, nrows, offset));
   if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -1412,6 +1445,7 @@ int dfb_train_step(dfb_handle h, size_t nrows, const uint64_t* offset, const uin
 int dfb_read_entries(dfb_handle h, const uint64_t* keys, size_t n, float* scal_out, int* has_V_out, float* V_out,
                      float* cg_out) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_read_entries");
   if (n == 0) return DFB_OK;
   if (!keys || !scal_out || !has_V_out) return h->fail(DFB_ERR_INVALID, "NULL argument");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -1466,6 +1500,7 @@ int dfb_shard_bounds(const uint64_t* keys, size_t n, uint32_t S, size_t* bounds)
 
 int dfb_dev_feacnt(dfb_handle h, const uint64_t* d_keys, size_t n, const float* d_cnt) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_dev_feacnt");
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));
@@ -1481,6 +1516,7 @@ int dfb_dev_feacnt(dfb_handle h, const uint64_t* d_keys, size_t n, const float* 
 static int dev_pull_rows_impl(dfb_handle h, const uint64_t* d_keys, size_t n, float* d_w_out, int* d_hasv_out,
                               int* d_hasv_out2, float* d_V_out) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_dev_pull_rows");
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));
@@ -1576,6 +1612,7 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
                            const int* d_hasv, const float* d_V, int is_train, float* d_gw_out, float* d_gV_out,
                            const SegDst* seg) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_dev_fm_step");
   DFB_CUDA(h, cudaSetDevice(h->device));
   cudaStream_t s = h->stream;
   const int ks = h->tab.ks, k = h->prm.V_dim;
@@ -1652,6 +1689,7 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
 int dfb_dev_push_rows(dfb_handle h, const uint64_t* d_keys, size_t n, const float* d_gw, const int* d_hasv,
                       const float* d_gV) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_dev_push_rows");
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (n == 0) return DFB_OK;
   DFB_TRY(ensure_key_ws(h, n));

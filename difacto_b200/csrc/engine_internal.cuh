@@ -27,6 +27,7 @@ struct dfb_engine {
   int scatter_sorted = 1;   // 1: atomic-free sorted reduction (deterministic); 0: red.global atomics
   int overlap_auc = 1;      // run the AUC kernels on the auxiliary stream, concurrently with the update
   int has_aux = 1;          // false after restoring a snapshot saved without aux data (sgd_updater.h:88)
+  int score_only = 0;       // kwarg score_only: V-only rows (tab.vonly), has_aux 0; restore, raw predict and reads only
   int restored_parts = 0;   // snapshot streams merged into the table since it was last empty (checkpoint.cu)
   int l2_hints = 1;         // per-load L2 eviction policies in the gather kernels
   int id_bits = 0;          // > 0: feature ids are < 2^id_bits (fixes the radix-sort bit range of the GPU localizer)
@@ -127,6 +128,12 @@ struct dfb_engine {
     return !force_generic && dfb::fm_fast_supported(prm.V_dim) && (!is_train || scatter_sorted);
   }
   int fail(int code, const std::string& msg) { err = msg; return code; }
+  // at the top of every entry point that trains, counts features, reads or writes rows, saves, prunes or shards: a
+  // scoring-only engine holds neither the AdaGrad half of a row nor, with bf16 rows, the V values a snapshot stores
+  int refuse_score_only(const char* call) {
+    return fail(DFB_ERR_INVALID, std::string(call) + " is not available on a score_only = 1 engine (it restores a "
+                                 "model and scores with dfb_predict_raw_*)");
+  }
   int cuda_fail(cudaError_t e, const char* what) {
     err = std::string(what) + ": " + cudaGetErrorString(e);
     return DFB_ERR_CUDA;
@@ -139,6 +146,10 @@ struct dfb_engine {
   do {                                                                     \
     cudaError_t _e = (call);                                               \
     if (_e != cudaSuccess) return (h)->cuda_fail(_e, #call);               \
+  } while (0)
+#define DFB_NOT_SCORE_ONLY(h, call)                                \
+  do {                                                             \
+    if ((h)->score_only) return (h)->refuse_score_only(call);      \
   } while (0)
 #define DFB_TRY(expr)              \
   do {                             \

@@ -66,7 +66,8 @@ uint64_t next_pow2(uint64_t x) {
 
 size_t round_up(size_t x, size_t g) { return (x + g - 1) / g * g; }
 
-size_t row_bytes(const dfb_engine* h) { return (size_t)h->tab.rs * sizeof(float); }
+// rs elements of 4 bytes, or of 2 in a scoring-only engine's bf16 rows
+size_t row_bytes(const dfb_engine* h) { return (size_t)h->tab.rs * (h->tab.vonly == 2 ? 2 : 4); }
 
 // maps physical memory up to `bytes` (a multiple of the granularity, at most the reservation) of the V-row pool;
 // false (nothing changed) when the memory cannot be had
@@ -156,7 +157,7 @@ int dfbh::capacity_create(dfb_engine* h) {
     if (!vpool_map(h, round_up((size_t)t.vcap * row_bytes(h), g.gran)))
       return h->fail(DFB_ERR_CUDA, "out of device memory for V_capacity V rows");
     t.V = reinterpret_cast<float*>(g.vbase);
-    t.Vcg = t.V + t.ks;
+    t.Vcg = t.vonly ? nullptr : t.V + t.ks;
   }
   if (g.on) {
     DFB_CUDA(h, cudaHostAlloc(&g.h_st, 2 * dfb_engine::Growth::kRing * sizeof(unsigned long long), cudaHostAllocDefault));

@@ -8,6 +8,8 @@
 // this shard's records, a scan ranks them, and k_rst_insert puts them into the table and the row pool.
 #include "dfb_device.cuh"
 
+#include <cuda_bf16.h>
+
 #include <cub/cub.cuh>
 
 namespace dfb {
@@ -128,7 +130,10 @@ __global__ void k_rst_mark(const unsigned* __restrict__ buf, const unsigned* __r
 }
 
 // one warp per kept record: insert the key (a key already present raises kErrCkptDup), write its scalars, and its
-// V / cg row at n_vrows + rank with the pad columns [V_dim, ks) zero in both halves
+// V / cg row at n_vrows + rank with the pad columns [V_dim, ks) zero in both halves.
+// VONLY (a scoring-only engine's table): the row is V alone at stride ks, 1 = fp32, 2 = bf16 rounded to nearest even
+// (NaN and Inf as __float2bfloat16_rn defines them); the record's cg words are not read.
+template <int VONLY>
 __global__ void k_rst_insert(Table t, const unsigned* __restrict__ buf, const unsigned* __restrict__ roff, size_t n,
                              int aux, int k, const unsigned long long* __restrict__ flags,
                              const unsigned long long* __restrict__ rank) {
@@ -170,10 +175,15 @@ __global__ void k_rst_insert(Table t, const unsigned* __restrict__ buf, const un
     }
     if (hv) {
       const unsigned* src = rec + fixw;
-      float* row = t.V + (size_t)vrow * t.rs;
-      for (int j = (int)l; j < t.ks; j += 32) {
-        row[j] = j < k ? __uint_as_float(src[j]) : 0.f;
-        row[t.ks + j] = (aux && j < k) ? __uint_as_float(src[k + j]) : 0.f;
+      if (VONLY == 2) {
+        __nv_bfloat16* row = reinterpret_cast<__nv_bfloat16*>(t.V) + (size_t)vrow * t.rs;
+        for (int j = (int)l; j < t.ks; j += 32) row[j] = __float2bfloat16_rn(j < k ? __uint_as_float(src[j]) : 0.f);
+      } else {
+        float* row = t.V + (size_t)vrow * t.rs;
+        for (int j = (int)l; j < t.ks; j += 32) {
+          row[j] = j < k ? __uint_as_float(src[j]) : 0.f;
+          if (VONLY == 0) row[t.ks + j] = (aux && j < k) ? __uint_as_float(src[k + j]) : 0.f;
+        }
       }
     }
   }
@@ -246,7 +256,10 @@ int launch_rst_chunk(Table& t, const unsigned* buf, const unsigned* roff, size_t
                                                               t.prog);
   size_t tb = tmp_bytes;
   if (cub::DeviceScan::ExclusiveSum(tmp, tb, flags, rank, (int)n, s) != cudaSuccess) return -1;
-  k_rst_insert<<<grid_cap(n, 8, num_sms() * 16), 256, 0, s>>>(t, buf, roff, n, aux, k, flags, rank);
+  const int grid = grid_cap(n, 8, num_sms() * 16);
+  if (t.vonly == 2) k_rst_insert<2><<<grid, 256, 0, s>>>(t, buf, roff, n, aux, k, flags, rank);
+  else if (t.vonly == 1) k_rst_insert<1><<<grid, 256, 0, s>>>(t, buf, roff, n, aux, k, flags, rank);
+  else k_rst_insert<0><<<grid, 256, 0, s>>>(t, buf, roff, n, aux, k, flags, rank);
   k_rst_count<<<1, 1, 0, s>>>(t.state, flags, rank, n);
   return 4;
 }

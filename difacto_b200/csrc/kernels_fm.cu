@@ -83,6 +83,14 @@ __device__ __forceinline__ void probe_raw(const FmView& v, unsigned long long id
   }
 }
 
+// a lane's 4 columns of a V row, at element offset `at` from the rows' base: one 16-byte load of fp32 elements, or
+// (BF16: a scoring-only engine's 2-byte rows) one 8-byte load widened to fp32
+template <bool BF16>
+__device__ __forceinline__ float4 load_vrow4(const float* base, long long at, uint64_t pol) {
+  if constexpr (BF16) return ldg_bf16x4_pol(reinterpret_cast<const unsigned short*>(base) + at, pol);
+  else return ldg128_pol(base + at, pol);
+}
+
 __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, DevProgress* prog) {
   __shared__ float red_s[32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -126,9 +134,10 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 #ifndef DFB_FM_MINBLOCKS32
 #define DFB_FM_MINBLOCKS32 DFB_FM_MINBLOCKS     // V_dim = 32 (tuning builds: 3 removes its ~130-byte spills)
 #endif
-template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false, bool BF16 = false>
 __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MINBLOCKS) k_fm_fast(FmBatch b, FmView v, PartArgs pa) {
   constexpr bool TRAIN = MODE == 1;
+  static_assert(!BF16 || (RAW && MODE == 0), "bf16 rows: the raw-id predict step only");
   static_assert(!(PAD && TRAIN), "the atomic scatter runs the exact widths only");
   static_assert(!RAW || MODE == 0 || MODE == 2, "raw ids: predict and emit only");
   constexpr int LPR = K / 4;                 // lanes per V row, one float4 each
@@ -219,7 +228,7 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
           const float x_t = __shfl_sync(kFull, x, t & 31);
           const bool ok = (t < cnt) && (vr_t >= 0) && act;
           xs[q] = ok ? x_t : 0.f;
-          vv[q] = ok ? ldg128_pol(v.vbase + (long long)vr_t * v.vstride + sub * 4, pol_v)
+          vv[q] = ok ? load_vrow4<BF16>(v.vbase, (long long)vr_t * v.vstride + sub * 4, pol_v)
                      : make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
@@ -310,9 +319,10 @@ __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MIN
 // ---------------------------------------------------------------------------------------
 constexpr int kLongWarps = 8;
 
-template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false>
+template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false, bool BF16 = false>
 __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v, int scan_rows) {
   static_assert(!RAW || MODE == 0 || MODE == 2, "raw ids: predict and emit only");
+  static_assert(!BF16 || (RAW && MODE == 0), "bf16 rows: the raw-id predict step only");
   constexpr int LPR = K / 4;
   constexpr int G = 32 / LPR;
   constexpr int UNR = (32 / G) < 8 ? (32 / G) : 8;
@@ -381,7 +391,7 @@ __global__ void __launch_bounds__(kLongWarps * 32) k_fm_long(FmBatch b, FmView v
             const float x_t = __shfl_sync(kFull, x, t & 31);
             const bool ok = (t < cnt) && (vr_t >= 0) && act;
             xs[q] = ok ? x_t : 0.f;
-            vv[q] = ok ? ldg128_pol(v.vbase + (long long)vr_t * v.vstride + sub * 4, pol_v)
+            vv[q] = ok ? load_vrow4<BF16>(v.vbase, (long long)vr_t * v.vstride + sub * 4, pol_v)
                        : make_float4(0.f, 0.f, 0.f, 0.f);
           }
   #pragma unroll
@@ -572,8 +582,9 @@ __global__ void k_grad_finalize_dense(int k, int ks, size_t nkeys, const int* ha
 
 inline bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
-// RAW: the raw-id kernels (launch_fm_raw): predict (MODE 0) or, in a training step, emit (MODE 2)
-template <int K, bool PAD, bool RAW = false>
+// RAW: the raw-id kernels (launch_fm_raw): predict (MODE 0) or, in a training step, emit (MODE 2).
+// BF16 (RAW predict only): the rows are a scoring-only engine's bf16 V rows
+template <int K, bool PAD, bool RAW = false, bool BF16 = false>
 int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const int threads = 256;
   size_t need = (b.nrows + 7) / 8;
@@ -581,7 +592,11 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   const bool hv = b.value != nullptr;
   PartArgs pa;
   memset(&pa, 0, sizeof(pa));
-  if constexpr (RAW) {
+  if constexpr (BF16) {
+    if (b.train) return -1;
+    if (hv) k_fm_fast<K, 0, true, PAD, true, true><<<grid, threads, 0, s>>>(b, v, pa);
+    else    k_fm_fast<K, 0, false, PAD, true, true><<<grid, threads, 0, s>>>(b, v, pa);
+  } else if constexpr (RAW) {
     if (b.train) {
       if (hv) k_fm_fast<K, 2, true, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
       else    k_fm_fast<K, 2, false, PAD, true><<<grid, threads, 0, s>>>(b, v, pa);
@@ -605,7 +620,10 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
     const int lgrid = (int)(b.nrows < (size_t)(num_sms() * 4) ? b.nrows : (size_t)(num_sms() * 4));
     int scan = 1;
     while (scan < kLongWarps * 32 && (size_t)lgrid * scan * 2 <= b.nrows) scan *= 2;
-    if constexpr (RAW) {
+    if constexpr (BF16) {
+      if (hv) k_fm_long<K, 0, true, PAD, true, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+      else    k_fm_long<K, 0, false, PAD, true, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
+    } else if constexpr (RAW) {
       if (b.train) {
         if (hv) k_fm_long<K, 2, true, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
         else    k_fm_long<K, 2, false, PAD, true><<<lgrid, kLongWarps * 32, 0, s>>>(b, v, scan);
@@ -653,12 +671,14 @@ int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& p
   });
 }
 
-int launch_fm_raw(const FmBatch& b, const FmView& v, cudaStream_t s) {
+int launch_fm_raw(const FmBatch& b, const FmView& v, bool bf16_rows, cudaStream_t s) {
   // training: the emit mode over the CSC view the GPU localizer already wrote
-  if (b.train && (!b.emit || b.occ_row != nullptr || b.occ_rowx != nullptr)) return -1;
+  if (b.train && (bf16_rows || !b.emit || b.occ_row != nullptr || b.occ_rowx != nullptr)) return -1;
   if (!aligned16(v.vbase) || v.vstride % 4 != 0) return -1;
   return with_lane_width(b.V_dim, [&](auto kc) {
     constexpr int K = decltype(kc)::value;
+    if (bf16_rows)
+      return b.V_dim == K ? launch_fast_k<K, false, true, true>(b, v, s) : launch_fast_k<K, true, true, true>(b, v, s);
     return b.V_dim == K ? launch_fast_k<K, false, true>(b, v, s) : launch_fast_k<K, true, true>(b, v, s);
   });
 }

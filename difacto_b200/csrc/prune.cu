@@ -68,6 +68,7 @@ extern "C" {
 
 int dfb_prune(dfb_handle h, float max_count, uint64_t* n_dropped) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_prune");
   if (!n_dropped) return h->fail(DFB_ERR_INVALID, "n_dropped is NULL");
   *n_dropped = 0;
   if (max_count != max_count) return h->fail(DFB_ERR_INVALID, "dfb_prune: max_count is NaN");

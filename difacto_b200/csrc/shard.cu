@@ -432,6 +432,7 @@ extern "C" {
 int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t max_nnz, size_t seg_keys,
                    size_t seg_nnz, size_t* mailbox_bytes) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_shard_init");
   if (h->shard) return h->fail(DFB_ERR_INVALID, "dfb_shard_init was already called");
   if (nranks < 1 || nranks > 8 || rank < 0 || rank >= nranks) return h->fail(DFB_ERR_INVALID, "1 <= nranks <= 8, 0 <= rank < nranks");
   if (max_rows == 0 || max_nnz == 0 || max_nnz > 0x7fffffffULL || max_rows > 0x7fffffffULL)

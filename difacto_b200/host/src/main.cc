@@ -12,6 +12,9 @@ int main(int argc, char* argv[]) {
   using namespace difacto;   // NOLINT
   if (argc < 2) {
     fprintf(stderr, "usage: difacto_b200 key1=val1 key2=val2 ...\n");
+    fprintf(stderr, "  task=predict model_in=M data_in=D [pred_out=P] [score_only=1 [V_storage=bf16]]: score a saved model;\n"
+                    "  score_only=1 loads it without its AdaGrad state (half the V-row memory, the same predictions),\n"
+                    "  V_storage=bf16 also stores V in bf16 (a quarter; predictions differ by bf16 rounding of V)\n");
     return 0;
   }
   try {

@@ -83,6 +83,12 @@ std::vector<std::pair<std::string, std::string>> SGDLearner::Settings(const SGDL
 // SGDLearner::Init, sgd_learner.cc:229-246
 KWArgs SGDLearner::Init(const KWArgs& kwargs) {
   KWArgs remain = param_.InitAllowUnknown(kwargs);
+  // score_only / V_storage are engine keys and reach dfb_create with the rest; the sharded store keeps the training
+  // layout in its shards, so a scoring-only model is scored on one GPU
+  if (param_.num_gpus > 1)
+    for (const auto& kv : kwargs)
+      if (kv.first == "score_only" && kv.second != "0")
+        throw ParamError("score_only = 1 needs num_gpus = 1 (the sharded predict keeps training-layout shards)");
   settings_ = Settings(param_, kwargs);
   auto* updater = new GpuSGDUpdater();
   std::shared_ptr<Updater> holder(updater);

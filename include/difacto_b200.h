@@ -106,6 +106,27 @@ typedef struct {
  *                         kernel, its chunks added in a fixed order (0: one warp per example whatever its length)
  *   force_generic (0)     1 = use the any-V_dim kernels even where a specialised one exists (tests).  Specialised
  *                         kernels exist for 0 <= V_dim <= 128 (the atomic scatter: V_dim in {8,16,32,64,128})
+ *   score_only (0)        1 = a scoring-only engine: it loads a model (dfb_restore*, any snapshot, with or without aux
+ *                         data, any M parts -> this shard) and scores it (dfb_predict_raw_*).  Its V rows hold V
+ *                         alone -- stride dfb_row_stride elements instead of twice that, no AdaGrad accumulators -- so
+ *                         the row pool takes half the memory (V_capacity / V_capacity_max count rows as before, and
+ *                         a restore grows the engine up to the maxima).  has_aux reads 0.  Also allowed:
+ *                         dfb_table_stats, dfb_row_bytes, dfb_id_range_get/set, dfb_sync, dfb_prefetch_raw, the
+ *                         Progress reads (dfb_wait_step, dfb_read_progress), dfb_evaluate / dfb_auc, the timing
+ *                         calls, dfb_destroy.  Every call that trains, counts features, validates, reads or writes
+ *                         rows, saves, prunes or shards returns DFB_ERR_INVALID with a message naming score_only
+ *                         and changes nothing: dfb_train_step*, dfb_train_step_raw*, dfb_push_feacnt, dfb_pull,
+ *                         dfb_push_grad, dfb_predict, dfb_calc_grad, dfb_read_entries, dfb_dev_*, dfb_snapshot*,
+ *                         dfb_prune, dfb_shard_init.  Needs 0 <= V_dim <= 128 and force_generic = 0 (DFB_ERR_PARAM
+ *                         otherwise): the predict step of other configurations is the validation step.
+ *                         The fp32 scoring engine's predictions and Progress are bit-identical to the training
+ *                         engine's predict step on the same model.
+ *   V_storage (fp32)      fp32 | bf16: the element type of a scoring-only engine's V rows.  bf16 halves the rows
+ *                         again (2 bytes per element): restore rounds every V value to the nearest bf16, ties to
+ *                         even (NaN and Inf as __float2bfloat16_rn defines them), the forward widens the elements
+ *                         back to fp32 (exact) and accumulates in fp32 in the fp32 kernels' order, so its outputs
+ *                         are bit-identical to an fp32 scoring engine's on a model whose V values were rounded so
+ *                         beforehand.  w stays fp32.  bf16 without score_only = 1 is DFB_ERR_PARAM.
  * Keys that are neither are returned through dfb_unknown_kwarg, mirroring the
  * "return the unconsumed kwargs" convention (updater.h:34, main.cc:25-31).
  * ------------------------------------------------------------------------------- */
@@ -119,6 +140,9 @@ uint64_t dfb_launch_count(dfb_handle h);
 /* number of keys / V rows currently stored, and the current (grown) key and V-row capacities */
 int dfb_table_stats(dfb_handle h, uint64_t* n_keys, uint64_t* n_vrows, uint64_t* capacity,
                     uint64_t* v_capacity);
+/* the bytes one V row takes in the row pool -- dfb_row_stride elements times 8 ([V|cg] of a training engine), 4
+ * (score_only, fp32) or 2 (score_only, V_storage = bf16) -- and n_vrows times that (either may be NULL) */
+int dfb_row_bytes(dfb_handle h, uint64_t* bytes_per_row, uint64_t* bytes_in_use);
 
 /* pinned host memory so that H2D/D2H copies are asynchronous DMA */
 int dfb_host_alloc(void** ptr, size_t bytes);
@@ -247,7 +271,9 @@ int dfb_train_step_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_
  *                          other async steps, and sees the updates of the training steps enqueued before it.
  *   dfb_predict_raw_dev    device buffers, enqueue only (the Progress accumulates as for dfb_train_step_raw_dev);
  *                          d_pred_out_or_null receives the predictions in stream order.
- * An engine that is a rank of the sharded store (dfb_shard_init) refuses both: DFB_ERR_INVALID. */
+ * An engine that is a rank of the sharded store (dfb_shard_init) refuses both: DFB_ERR_INVALID.
+ * These are the steps a score_only = 1 engine runs: on fp32 rows the same kernels at the V-only row stride, on bf16
+ * rows (V_storage = bf16) instantiations of them that differ in the row load alone. */
 int dfb_predict_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
                           const float* value_or_null, const float* label_or_null, float* pred_out_or_null);
 int dfb_predict_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
@@ -310,7 +336,11 @@ int dfb_read_entries(dfb_handle h, const uint64_t* keys, size_t n, float* scal_o
  * message says the table was cleared -- so that the caller can retry.  dfb_snapshot_write changes nothing, also
  * when write_fn fails.
  * dfb_snapshot / dfb_restore are the same over one memory buffer (dfb_snapshot_size bytes); dfb_restore needs an
- * empty table (refused without clearing anything otherwise). */
+ * empty table (refused without clearing anything otherwise).
+ * A score_only = 1 engine restores the same streams into V-only rows (the records' cg and, for the engine's has_aux,
+ * their aux data are skipped; V_storage = bf16 rounds V to nearest even) and reports has_aux 0; dfb_snapshot_size,
+ * dfb_snapshot, dfb_snapshot_write and dfb_snapshot_begin are refused on it (DFB_ERR_INVALID): it no longer holds
+ * what the format stores. */
 typedef int (*dfb_write_fn)(void* ctx, const void* buf, size_t bytes);   /* 0 = ok */
 typedef size_t (*dfb_read_fn)(void* ctx, void* buf, size_t cap);       /* bytes read, 0 = end, (size_t)-1 = error */
 int dfb_snapshot_write(dfb_handle h, int save_aux, size_t chunk_bytes, dfb_write_fn write_fn, void* ctx);
@@ -361,7 +391,8 @@ int dfb_id_range_set(dfb_handle h, int bits);
  * new keys.  Like dfb_snapshot_begin it waits for every stream of the handle and runs between steps: during a sharded
  * step (dfb_shard_begin_* .. dfb_shard_phase(4)) it is DFB_ERR_INVALID.  A frozen snapshot is a copy and is not
  * changed.  The table is rebuilt in place with a workspace of 32 bytes per kept entry, taken before the table is
- * touched: DFB_ERR_CAPACITY when it cannot be had, and then nothing has changed. */
+ * touched: DFB_ERR_CAPACITY when it cannot be had, and then nothing has changed.  Refused on a score_only = 1
+ * engine (DFB_ERR_INVALID): prune the model where it is trained. */
 int dfb_prune(dfb_handle h, float max_count, uint64_t* n_dropped);
 
 /* ---------------------------------------------------------------------------------
@@ -430,7 +461,8 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
  * per-example partial interaction sums (see csrc/kernels_shard.cu); nothing is synchronised with the host.
  *   dfb_shard_init     allocate this rank's mailbox (capacity: max_rows x max_nnz per minibatch; seg_keys /
  *                      seg_nnz = capacity of one (worker, owner) key segment, 0 = twice the even share).  Needs
- *                      0 <= V_dim <= 128, scatter=sorted and force_generic=0 (DFB_ERR_INVALID otherwise)
+ *                      0 <= V_dim <= 128, scatter=sorted and force_generic=0 (DFB_ERR_INVALID otherwise); a
+ *                      score_only = 1 engine is refused (the shards keep the training layout)
  *   dfb_shard_export   the mailbox pointer (peers in the same process) and its CUDA IPC handle (peers in
  *                      other processes open it with dfb_peer_open)
  *   dfb_shard_connect  the peers' mailbox pointers, indexed by rank (entry [rank] is ignored)
