@@ -40,7 +40,7 @@ EXPORTS = [
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
     "dfb_predict_raw_async", "dfb_predict_raw_dev", "dfb_shard_predict_async", "dfb_shard_begin_predict_async",
-    "dfb_row_bytes",
+    "dfb_row_bytes", "dfb_growth_stats",
 ]
 
 _LIB = None
@@ -69,6 +69,7 @@ def lib():
         L.dfb_launch_count.argtypes = [vp]
         L.dfb_table_stats.argtypes = [vp] + [C.POINTER(u64)] * 4
         L.dfb_row_bytes.argtypes = [vp] + [C.POINTER(u64)] * 2
+        L.dfb_growth_stats.argtypes = [vp] + [C.POINTER(u64)] * 2
         L.dfb_host_alloc.argtypes = [C.POINTER(vp), sz]
         L.dfb_host_free.argtypes = [vp]
         L.dfb_push_feacnt.argtypes = [vp, vp, sz, vp]
@@ -212,7 +213,8 @@ class Engine:
 
     The keyword arguments are dfb_create's keys (include/difacto_b200.h).  table_capacity / V_capacity are the initial
     capacities; with table_capacity_max / V_capacity_max above them the table and the V-row pool grow on demand, and
-    table_stats() reports the current capacities.  score_only=True (optionally V_storage="bf16") makes a scoring-only
+    table_stats() reports the current capacities; shard_growth=1 lets such an engine be a rank of the fused sharded
+    store, whose owners then grow by the keys they receive.  score_only=True (optionally V_storage="bf16") makes a scoring-only
     engine: restore and predict_raw* only, V rows without their AdaGrad halves; what it refuses raises DfbError."""
 
     def __init__(self, **kwargs):
@@ -263,6 +265,12 @@ class Engine:
         a, b, c, d = C.c_uint64(), C.c_uint64(), C.c_uint64(), C.c_uint64()
         self._ck(self.L.dfb_table_stats(self.h, C.byref(a), C.byref(b), C.byref(c), C.byref(d)))
         return dict(n_keys=a.value, n_vrows=b.value, capacity=c.value, v_capacity=d.value)
+
+    def growth_stats(self):
+        """(calls that grew the table or the V-row pool, sharded growth decisions that waited for the device)"""
+        a, b = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.dfb_growth_stats(self.h, C.byref(a), C.byref(b)))
+        return a.value, b.value
 
     def row_bytes(self):
         """(bytes one V row takes in the row pool, n_vrows times that)"""

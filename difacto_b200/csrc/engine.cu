@@ -688,6 +688,7 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     else if (k == "l2_hints") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->l2_hints = (int)x; }
     else if (k == "id_bits") { if (!need_int(0, 64)) { delete h; return DFB_ERR_PARAM; } h->id_bits = (int)x; }
     else if (k == "shard_timeout_ms") { if (!need_int(1, 3600000)) { delete h; return DFB_ERR_PARAM; } h->shard_timeout_ms = x; }
+    else if (k == "shard_growth") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->shard_growth = (int)x; }
     else if (k == "score_only") { if (!need_int(0, 1)) { delete h; return DFB_ERR_PARAM; } h->score_only = (int)x; }
     else if (k == "V_storage") {
       if (v == "fp32") v_bf16 = false;
@@ -851,6 +852,13 @@ int dfb_row_bytes(dfb_handle h, uint64_t* bytes_per_row, uint64_t* bytes_in_use)
   DFB_TRY(dfb_table_stats(h, nullptr, &n_vrows, nullptr, nullptr));
   if (bytes_per_row) *bytes_per_row = rb;
   if (bytes_in_use) *bytes_in_use = n_vrows * rb;
+  return DFB_OK;
+}
+
+int dfb_growth_stats(dfb_handle h, uint64_t* growths, uint64_t* host_waits) {
+  if (!h) return DFB_ERR_INVALID;
+  if (growths) *growths = h->grow.n_growths;
+  if (host_waits) *host_waits = h->grow.n_waits;
   return DFB_OK;
 }
 

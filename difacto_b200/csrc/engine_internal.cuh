@@ -120,7 +120,20 @@ struct dfb_engine {
     uint64_t at_k[kRing] = {}, at_v[kRing] = {};    // the bound totals when the copy was enqueued
     uint64_t head = 0, seq = 0;                     // ring entries [head, seq) are in flight
     uint64_t known_k = 0, known_v = 0, known_at_k = 0, known_at_v = 0, total_k = 0, total_v = 0;
+    // sharded steps (shard_growth = 1): each one adds its worst case to the totals and is made exact once k_shard_count
+    // has stored the keys its owner received.  calls numbers the bounds added, so that a correction reaches exactly
+    // the copies whose totals include the corrected bound.
+    uint64_t calls = 0, at_call[kRing] = {}, known_at_call = 0;
+    unsigned long long* h_rcv = nullptr;            // pinned, mapped [kRing]: the received keys of one sharded step
+    unsigned long long* d_rcv = nullptr;            // its device address
+    cudaEvent_t rev[kRing] = {};
+    uint64_t r_call[kRing] = {}, r_worst[kRing] = {};
+    bool r_v[kRing] = {};                           // the step's bound was added to the V rows' total too
+    uint64_t rhead = 0, rseq = 0;                   // entries [rhead, rseq) are not yet exact
+    // calls that grew the table or the pool; host waits for a sharded step's count (dfb_growth_stats)
+    uint64_t n_growths = 0, n_waits = 0;
   } grow;
+  int shard_growth = 0;     // kwarg shard_growth: a growing engine may be a rank of the fused sharded store
 
   // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (0 <= V_dim <= 128) and,
   // when it trains, the atomic-free sorted gradient reduction
@@ -206,13 +219,23 @@ void capacity_destroy(dfb_engine* h);
 // waits for the device, and a failed allocation keeps the current table and pool (a step that really overflows them
 // reports DFB_ERR_CAPACITY).  Does nothing on an engine that cannot grow.
 int reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows);
+// the sharded step's growth (shard_growth = 1), in phase 1 before the lookup.  shard_rcv_slot: where k_shard_count
+// stores the keys this owner receives in the step, or NULL when nothing can grow (then nothing below is called).
+// reserve_shard, after that count is enqueued on counted_on: grows the table and the pool when the known counts plus
+// the bounds in flight -- each step's received keys once counted, `worst` before -- could exceed their capacities,
+// waiting for this step's count first when the worst case does not fit.  *rehashed: the table was rebuilt on
+// h->stream, which the lookup must wait for.  shard_counts_copy, after the step's InitV: the counts the next
+// decision starts from.
+int shard_rcv_slot(dfb_engine* h, unsigned long long** slot);
+int reserve_shard(dfb_engine* h, cudaStream_t counted_on, uint64_t worst, bool vrows, bool* rehashed);
+int shard_counts_copy(dfb_engine* h);
 // a copy of the table's slots (cap entries) and of V rows [0, n_vrows) in fresh stream-ordered device memory, made
 // on h->stream and waited for; DFB_ERR_CAPACITY with nothing allocated when the memory cannot be had.  The copy keeps
 // cap, mask, ks and rs, has vcap = n_vrows and no state or progress: the snapshot writer's view of a table.
 int table_copy(dfb_engine* h, uint64_t n_vrows, dfb::Table* out);
 void table_copy_free(dfb::Table* t, cudaStream_t s);   // stream-ordered on s
 // after a dfb_prune (which waited for every stream): the table holds exactly n_keys keys and n_vrows V rows, and no
-// inserting call is in flight
+// inserting call or sharded step is in flight
 void counts_known(dfb_engine* h, uint64_t n_keys, uint64_t n_vrows);
 void frozen_destroy(dfb_frozen_s* f);   // checkpoint.cu: frees the copy after its stream's work
 int drain(dfb_engine* h);               // checkpoint.cu: wait for everything enqueued on any of the handle's streams

@@ -163,6 +163,11 @@ int dfbh::capacity_create(dfb_engine* h) {
     DFB_CUDA(h, cudaHostAlloc(&g.h_st, 2 * dfb_engine::Growth::kRing * sizeof(unsigned long long), cudaHostAllocDefault));
     for (auto& ev : g.ev) DFB_CUDA(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
   }
+  if (g.on && h->shard_growth) {
+    DFB_CUDA(h, cudaHostAlloc(&g.h_rcv, dfb_engine::Growth::kRing * sizeof(unsigned long long), cudaHostAllocMapped));
+    DFB_CUDA(h, cudaHostGetDevicePointer(reinterpret_cast<void**>(&g.d_rcv), g.h_rcv, 0));
+    for (auto& ev : g.rev) DFB_CUDA(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+  }
   return 0;
 }
 
@@ -189,15 +194,38 @@ void dfbh::capacity_destroy(dfb_engine* h) {
   h->tab.V = h->tab.Vcg = nullptr;
   if (g.h_st) cudaFreeHost(g.h_st);
   for (auto& ev : g.ev) if (ev) cudaEventDestroy(ev);
+  if (g.h_rcv) cudaFreeHost(g.h_rcv);
+  for (auto& ev : g.rev) if (ev) cudaEventDestroy(ev);
 }
 
-int dfbh::reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows) {
+namespace {
+
+bool can_grow(const dfb_engine* h) {
+  const dfb_engine::Growth& g = h->grow;
+  const Table& t = h->tab;
+  return g.on && (t.max_keys < g.tab_max || (g.vbase && t.vcap < g.v_max));
+}
+
+// takes in what the device has finished: the received-key counts of sharded steps (each replaces its step's worst case
+// in the totals, and in every copy taken after that bound was added), then the newest completed copy of the counts
+int fold(dfb_engine* h) {
   dfb_engine::Growth& g = h->grow;
-  Table& t = h->tab;
-  if (!g.on || (t.max_keys >= g.tab_max && (t.vcap >= g.v_max || !g.vbase))) return 0;   // nothing can grow
   constexpr int R = dfb_engine::Growth::kRing;
-  new_keys = std::min<uint64_t>(new_keys, 1ULL << 32);    // above any capacity (a snapshot header is outside input)
-  new_vrows = std::min<uint64_t>(new_vrows, 1ULL << 32);
+  while (g.rhead < g.rseq) {
+    const int r = (int)(g.rhead % R);
+    const cudaError_t e = cudaEventQuery(g.rev[r]);
+    if (e == cudaErrorNotReady) break;
+    if (e != cudaSuccess) return h->cuda_fail(e, "cudaEventQuery(received keys)");
+    const uint64_t d = g.r_worst[r] - std::min<uint64_t>(g.h_rcv[r], g.r_worst[r]);
+    const uint64_t dv = g.r_v[r] ? d : 0;
+    g.total_k -= d; g.total_v -= dv;
+    for (uint64_t i = g.head; i < g.seq; ++i) {
+      const int c = (int)(i % R);
+      if (g.at_call[c] > g.r_call[r]) { g.at_k[c] -= d; g.at_v[c] -= dv; }
+    }
+    if (g.known_at_call > g.r_call[r]) { g.known_at_k -= d; g.known_at_v -= dv; }
+    g.rhead++;
+  }
   // the copies complete in stream order: take the newest one that has
   while (g.head < g.seq) {
     const int r = (int)(g.head % R);
@@ -205,33 +233,115 @@ int dfbh::reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows) {
     if (e == cudaErrorNotReady) break;
     if (e != cudaSuccess) return h->cuda_fail(e, "cudaEventQuery(table counts)");
     g.known_k = g.h_st[2 * r]; g.known_v = g.h_st[2 * r + 1];
-    g.known_at_k = g.at_k[r]; g.known_at_v = g.at_v[r];
+    g.known_at_k = g.at_k[r]; g.known_at_v = g.at_v[r]; g.known_at_call = g.at_call[r];
     g.head++;
   }
-  const uint64_t need_k = g.known_k + (g.total_k - g.known_at_k) + new_keys;
-  const uint64_t need_v = g.known_v + (g.total_v - g.known_at_v) + new_vrows;
-  // geometric: at least double, and at least the bound -- so a capacity stays below twice what it had to hold
+  return 0;
+}
+
+// the counts the table may reach: the last known ones plus every bound added since (and new_* not added yet)
+uint64_t need_keys(const dfb_engine::Growth& g, uint64_t new_keys = 0) { return g.known_k + (g.total_k - g.known_at_k) + new_keys; }
+uint64_t need_vrows(const dfb_engine::Growth& g, uint64_t new_vrows = 0) { return g.known_v + (g.total_v - g.known_at_v) + new_vrows; }
+
+bool short_of(const dfb_engine* h) {
+  const dfb_engine::Growth& g = h->grow;
+  const Table& t = h->tab;
+  return (need_keys(g) > t.max_keys && t.max_keys < g.tab_max) ||
+         (g.vbase && need_vrows(g) > t.vcap && t.vcap < g.v_max);
+}
+
+// geometric: at least double, and at least the need -- so a capacity stays below twice what it had to hold
+int grow_to_need(dfb_engine* h, uint64_t new_keys = 0, uint64_t new_vrows = 0) {
+  dfb_engine::Growth& g = h->grow;
+  Table& t = h->tab;
+  const uint64_t need_k = need_keys(g, new_keys), need_v = need_vrows(g, new_vrows);
+  const uint64_t k0 = t.max_keys, v0 = t.vcap;
   if (need_k > t.max_keys && t.max_keys < g.tab_max)
     DFB_TRY(grow_table(h, std::min(g.tab_max, std::max(need_k, 2 * t.max_keys))));
   if (g.vbase && need_v > t.vcap && t.vcap < g.v_max) grow_pool(h, std::min(g.v_max, std::max(need_v, 2 * t.vcap)));
-  if (g.seq - g.head < (uint64_t)R) {
-    const int r = (int)(g.seq % R);
-    DFB_CUDA(h, cudaMemcpyAsync(g.h_st + 2 * r, t.state, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
-                                h->stream));
-    DFB_CUDA(h, cudaEventRecord(g.ev[r], h->stream));
-    g.at_k[r] = g.total_k; g.at_v[r] = g.total_v;
-    g.seq++;
-  }
+  if (t.max_keys != k0 || t.vcap != v0) g.n_growths++;
+  return 0;
+}
+
+// a copy of {n_keys, n_vrows} as they are at this point of h->stream, with the bound totals it corresponds to
+int enqueue_copy(dfb_engine* h) {
+  dfb_engine::Growth& g = h->grow;
+  constexpr int R = dfb_engine::Growth::kRing;
+  if (g.seq - g.head >= (uint64_t)R) return 0;
+  const int r = (int)(g.seq % R);
+  DFB_CUDA(h, cudaMemcpyAsync(g.h_st + 2 * r, h->tab.state, 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost,
+                              h->stream));
+  DFB_CUDA(h, cudaEventRecord(g.ev[r], h->stream));
+  g.at_k[r] = g.total_k; g.at_v[r] = g.total_v; g.at_call[r] = g.calls;
+  g.seq++;
+  return 0;
+}
+
+}  // namespace
+
+int dfbh::reserve(dfb_engine* h, uint64_t new_keys, uint64_t new_vrows) {
+  if (!can_grow(h)) return 0;
+  dfb_engine::Growth& g = h->grow;
+  new_keys = std::min<uint64_t>(new_keys, 1ULL << 32);    // above any capacity (a snapshot header is outside input)
+  new_vrows = std::min<uint64_t>(new_vrows, 1ULL << 32);
+  DFB_TRY(fold(h));
+  DFB_TRY(grow_to_need(h, new_keys, new_vrows));
+  DFB_TRY(enqueue_copy(h));
   g.total_k += new_keys;
   g.total_v += new_vrows;
+  g.calls++;
   return 0;
+}
+
+int dfbh::shard_rcv_slot(dfb_engine* h, unsigned long long** slot) {
+  *slot = nullptr;
+  if (!h->shard_growth || !can_grow(h)) return 0;
+  dfb_engine::Growth& g = h->grow;
+  constexpr int R = dfb_engine::Growth::kRing;
+  // a full ring: the oldest count is that of a step kRing steps back, whose phase 0 every rank has enqueued
+  if (g.rseq - g.rhead >= (uint64_t)R) {
+    DFB_CUDA(h, cudaEventSynchronize(g.rev[g.rhead % R]));
+    g.n_waits++;
+    DFB_TRY(fold(h));
+  }
+  *slot = g.d_rcv + g.rseq % R;
+  return 0;
+}
+
+int dfbh::reserve_shard(dfb_engine* h, cudaStream_t counted_on, uint64_t worst, bool vrows, bool* rehashed) {
+  dfb_engine::Growth& g = h->grow;
+  constexpr int R = dfb_engine::Growth::kRing;
+  const int r = (int)(g.rseq % R);
+  DFB_CUDA(h, cudaEventRecord(g.rev[r], counted_on));
+  g.r_call[r] = g.calls++; g.r_worst[r] = worst; g.r_v[r] = vrows;
+  g.rseq++;
+  g.total_k += worst;
+  if (vrows) g.total_v += worst;
+  DFB_TRY(fold(h));
+  // the worst case does not fit: wait for this step's count.  It waits only for every worker's structure of this step
+  // (phase 0, enqueued by each rank before its phase 1) and for the poller in front of it, which times out.
+  if (short_of(h) && g.rhead < g.rseq) {
+    DFB_CUDA(h, cudaEventSynchronize(g.rev[r]));
+    g.n_waits++;
+    DFB_TRY(fold(h));
+  }
+  const Entry* before = h->tab.tab;
+  DFB_TRY(grow_to_need(h));
+  *rehashed = h->tab.tab != before;
+  return 0;
+}
+
+int dfbh::shard_counts_copy(dfb_engine* h) {
+  if (!h->shard_growth || !can_grow(h)) return 0;
+  return enqueue_copy(h);
 }
 
 void dfbh::counts_known(dfb_engine* h, uint64_t n_keys, uint64_t n_vrows) {
   dfb_engine::Growth& g = h->grow;
-  g.head = g.seq;                       // the copies in flight are complete, and older than these counts
+  g.head = g.seq;                       // the copies and counts in flight are complete, and older than these counts
+  g.rhead = g.rseq;
   g.known_k = n_keys; g.known_v = n_vrows;
-  g.known_at_k = g.total_k; g.known_at_v = g.total_v;
+  g.known_at_k = g.total_k; g.known_at_v = g.total_v; g.known_at_call = g.calls;
 }
 
 int dfbh::table_copy(dfb_engine* h, uint64_t n_vrows, Table* out) {

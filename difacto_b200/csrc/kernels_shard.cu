@@ -400,6 +400,18 @@ __global__ void __launch_bounds__(256) k_shard_lookup(Table t, LookupArgs a, int
   }
 }
 
+// the keys this owner received in one step: the sum over the workers' segments (each as k_shard_lookup reads it),
+// stored to host memory.  A growing owner bounds the step's new keys and new V rows by it (growth.cu, reserve_shard).
+__global__ void k_shard_count(LookupArgs a, unsigned long long* out) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  unsigned long long n = 0;
+  for (int r = 0; r < a.S; ++r) {
+    const unsigned long long k = a.hdr[r]->nkeys;
+    n += k < a.Kseg ? k : a.Kseg;
+  }
+  *out = n;
+}
+
 // Pull (Store::Pull -> SGDUpdater::Get, sgd_updater.cc:41-62) of all workers' key segments at once: {w, V-row index} of
 // every resolved slot -- taken AFTER the previous step's updates and this step's Update(kFeaCount), while the slots
 // themselves were resolved earlier (k_shard_lookup runs beside the previous step's update: open addressing without
@@ -537,6 +549,11 @@ int launch_shard_lookup(Table& t, const LookupArgs& a, int r, bool insert, unsig
   const int grid = grid_cap(a.Kseg, 256 * 2, num_sms() * 64);
   if (insert) k_shard_lookup<true><<<grid, 256, 0, s>>>(t, a, r, conf);
   else        k_shard_lookup<false><<<grid, 256, 0, s>>>(t, a, r, conf);
+  return 1;
+}
+
+int launch_shard_count(const LookupArgs& a, unsigned long long* out, cudaStream_t s) {
+  k_shard_count<<<1, 32, 0, s>>>(a, out);
   return 1;
 }
 

@@ -40,6 +40,7 @@ struct ShardState {
   cudaStream_t w_stream = nullptr, f_stream = nullptr, l_stream = nullptr;
   cudaEvent_t ev_struct[2] = {}, ev_part[2] = {}, ev_reduce[2] = {}, ev_auc[2] = {}, ev_upd[2] = {}, ev_fin[2] = {},
               ev_lookup[2] = {};
+  cudaEvent_t ev_grow = nullptr;     // a rehash on stream O, which the lookup of the same step waits for
   uint64_t step = 0;
   dfb_engine::LocSet L;
   DevBuf wb, rowcnt, pred[2];    // wb: ShardBounds [2] by step parity (the AUC of step t reads it beside step t+1)
@@ -215,6 +216,22 @@ int shard_phase(dfb_engine* h, int phase) {
     la.hdr[r] = hdr[r];
     la.keys[r] = lay.at<uint64_t>(mine, lay.off_keys, lay.str_keys, d, r);
   }
+  if (is_train || push_cnt) {
+    // a growing owner: count the keys this step brings (all workers' segments are in place after the poller), grow
+    // before they are inserted.  A rehash runs on stream O after the previous step's update, which still addresses
+    // the old slots; this step's lookup and everything after it take the new table.
+    unsigned long long* rcv = nullptr;
+    DFB_TRY(dfbh::shard_rcv_slot(h, &rcv));
+    if (rcv) {
+      h->launches += launch_shard_count(la, rcv, L);
+      bool rehashed = false;
+      DFB_TRY(dfbh::reserve_shard(h, L, (uint64_t)S * Kseg, is_train != 0, &rehashed));
+      if (rehashed) {
+        DFB_CUDA(h, cudaEventRecord(sh.ev_grow, O));
+        DFB_CUDA(h, cudaStreamWaitEvent(L, sh.ev_grow, 0));
+      }
+    }
+  }
   {
     StageTimer tm_lk(h, 0, L);
     // a validation / prediction batch must not grow the table (a missing entry reads as w = 0, no V)
@@ -352,6 +369,7 @@ int shard_phase(dfb_engine* h, int phase) {
   // which the reference's server would have met them
   if (is_train) h->launches += launch_initv(h->tab, h->prm, la.slot, (size_t)S * Kseg, nullptr, flags, ws, O);
   DFB_DBG(h, "InitV");
+  if (is_train || push_cnt) DFB_TRY(dfbh::shard_counts_copy(h));
   tm_upd.stop();
   DFB_CUDA(h, cudaEventRecord(sh.ev_upd[d], O));
   }
@@ -401,6 +419,7 @@ void dfbh::shard_destroy(dfb_engine* h) {
   if (sh->w_stream) cudaStreamDestroy(sh->w_stream);
   if (sh->f_stream) cudaStreamDestroy(sh->f_stream);
   if (sh->l_stream) cudaStreamDestroy(sh->l_stream);
+  if (sh->ev_grow) cudaEventDestroy(sh->ev_grow);
   cudaEvent_t* evs[] = {sh->ev_struct, sh->ev_part, sh->ev_reduce, sh->ev_auc, sh->ev_upd, sh->ev_fin, sh->ev_lookup};
   for (auto* e : evs) for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]);
   DevBuf* bufs[] = {&sh->L.keys, &sh->L.lidx, &sh->L.cnt, &sh->L.occ_sorted, &sh->L.col_start, &sh->L.col_end, &sh->L.scal,
@@ -441,10 +460,12 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   if (!h->sorted_path())
     return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in 0..128, scatter=sorted and no force_generic "
                                     "(other configurations: the all_to_all ShardedStore)");
-  // an owner's per-step insertion bound is only known on the host as S x seg_keys: far too much headroom to reserve
-  if (h->grow.on)
+  // a growing rank bounds each step's insertions by the keys its owner received, counted on the device
+  // (shard_growth = 1, growth.cu); without that opt-in the store keeps fixed capacities
+  if (h->grow.on && !h->shard_growth)
     return h->fail(DFB_ERR_INVALID, "the fused sharded store does not grow its shards: create the engine with "
-                                    "table_capacity_max = table_capacity and V_capacity_max = V_capacity");
+                                    "table_capacity_max = table_capacity and V_capacity_max = V_capacity, or with "
+                                    "shard_growth = 1");
   DFB_CUDA(h, cudaSetDevice(h->device));
   ShardState* sh = new ShardState();
   h->shard = sh;
@@ -472,6 +493,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   for (auto* ev : evs)
     for (int i = 0; i < 2; ++i)
       if ((e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
+  if ((e = cudaEventCreateWithFlags(&sh->ev_grow, cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
   const size_t tot = (size_t)nranks * Kseg;
   int rc = 0;
   if ((rc = h->ensure(sh->wb, 2 * sizeof(ShardBounds))) || (rc = h->ensure(sh->slot[0], tot * 4)) || (rc = h->ensure(sh->slot[1], tot * 4)) || (rc = h->ensure(sh->w, tot * 4)) ||

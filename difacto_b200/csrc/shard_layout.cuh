@@ -124,6 +124,8 @@ int launch_shard_subcsr(const uint64_t* offset, const uint32_t* lidx, const floa
 int launch_shard_reduce(const ReduceArgs& a, cudaStream_t s);
 // one launch per worker, in rank order (conf / vsave: [S][Kseg] flags and [S][Kseg][ks] saved rows; unused when stamp == 0)
 int launch_shard_lookup(Table& t, const LookupArgs& a, int r, bool insert, unsigned char* conf, cudaStream_t s);
+// the keys all workers' segments of this step bring (the sum of min(nkeys, Kseg)) -> *out (host-mapped memory)
+int launch_shard_count(const LookupArgs& a, unsigned long long* out, cudaStream_t s);
 int launch_shard_pull(Table& t, const LookupArgs& a, const unsigned char* conf, float* vsave, cudaStream_t s);
 int launch_shard_done(DevProgress* src_prog, DevProgress* main_prog, double* pen_dst, unsigned long long* flag_dst,
                       unsigned long long value, cudaStream_t s);

@@ -77,7 +77,20 @@ typedef struct {
  *                         without waiting for the device.  Capacities stay below about twice the keys plus the bounds
  *                         of the steps in flight.  A growth that cannot get memory keeps the current capacities; a
  *                         call reports DFB_ERR_CAPACITY exactly when it overflows them.  With both maxima at their
- *                         defaults nothing grows.  The fused sharded store refuses an engine that can grow.
+ *                         defaults nothing grows.  The fused sharded store refuses an engine that can grow unless
+ *                         shard_growth = 1.
+ *   shard_growth (0)      0 | 1: 1 lets an engine that can grow (a maximum above its capacity) be a rank of the fused
+ *                         sharded store (dfb_shard_init).  Before a training or feature-count step inserts, the owner
+ *                         counts on the device the keys every worker's segment brings it (one 1-thread kernel on its
+ *                         lookup stream) and grows to max(2 x current, the counts it knows + the keys received in the
+ *                         steps in flight), capped at the maxima.  The host waits for that count only when the worst
+ *                         case (nranks x seg_keys per step in flight) does not fit -- so a rank waits on every training
+ *                         step until its headroom reaches nranks x seg_keys.  The wait covers every worker's phase 0 of
+ *                         the step, and the poller in front of it times out after shard_timeout_ms.  A
+ *                         rehash runs on the owner stream after the previous step's update, and that step's lookup
+ *                         waits for it.  Results are bit-identical to pre-sized ranks; DFB_ERR_CAPACITY comes in the
+ *                         same step and rank as on ranks pre-sized to the maxima.  Validation and predict steps never
+ *                         grow.  An engine whose capacities equal its maxima launches exactly what a fixed one does.
  *   compute_auc (1)       evaluate AUC on device each step (sgd_learner.cc:150-153)
  *   scatter (sorted)      sorted = gradient reduced per key through a stable radix-sorted CSC view of
  *                         the batch, fused with the FTRL/AdaGrad step (no atomics, bit-reproducible,
@@ -143,6 +156,9 @@ int dfb_table_stats(dfb_handle h, uint64_t* n_keys, uint64_t* n_vrows, uint64_t*
 /* the bytes one V row takes in the row pool -- dfb_row_stride elements times 8 ([V|cg] of a training engine), 4
  * (score_only, fp32) or 2 (score_only, V_storage = bf16) -- and n_vrows times that (either may be NULL) */
 int dfb_row_bytes(dfb_handle h, uint64_t* bytes_per_row, uint64_t* bytes_in_use);
+/* calls that grew the table or the V-row pool so far, and how often a sharded step's growth decision waited for the
+ * device (shard_growth = 1: the worst case did not fit); either may be NULL */
+int dfb_growth_stats(dfb_handle h, uint64_t* growths, uint64_t* host_waits);
 
 /* pinned host memory so that H2D/D2H copies are asynchronous DMA */
 int dfb_host_alloc(void** ptr, size_t bytes);
