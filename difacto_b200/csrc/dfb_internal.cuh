@@ -225,7 +225,10 @@ size_t l2_bytes();
 
 // ---- launchers (kernels_fm.cu) ----
 // returns number of kernel launches performed, or <0 on invalid configuration
-int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s);
+// kLaunchRefused: the device refused the generic kernel's launch (its error in *launch_err when given)
+constexpr int kLaunchRefused = -2;
+int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s,
+              cudaError_t* launch_err = nullptr);
 // predict only, on raw ids (b.ids): the specialised kernels probe the table (v.tab) for each nonzero's key instead of
 // reading a pulled view; v.vbase / vstride = the table rows.  -1 when V_dim has no specialised kernels.
 // bf16_rows (predict only; a scoring-only engine with V_storage = bf16): v.vbase points at bf16 elements and vstride

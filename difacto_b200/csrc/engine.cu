@@ -196,6 +196,13 @@ int dfbh::prof_drain(dfb_engine* h) {
 }
 using dfbh::prof_drain;
 
+// the error of a launch_fm that returned nl < 0
+static int fm_launch_fail(dfb_engine* h, int nl, cudaError_t e) {
+  if (nl == dfb::kLaunchRefused)
+    return h->fail(DFB_ERR_CUDA, std::string("the FM forward launch failed: ") + cudaGetErrorString(e));
+  return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+}
+
 namespace {
 
 // the fused minibatch on device-resident inputs (everything enqueued on h->stream)
@@ -319,8 +326,9 @@ int step_dev(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, con
   }
   if (nrows) {
     StageTimer tm(h, 1);
-    const int nl = probe ? launch_fm_raw(b, v, false, s) : launch_fm(b, v, h->force_generic, s);
-    if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+    cudaError_t le = cudaSuccess;
+    const int nl = probe ? launch_fm_raw(b, v, false, s) : launch_fm(b, v, h->force_generic, s, &le);
+    if (nl < 0) return fm_launch_fail(h, nl, le);
     h->launches += nl;
   }
   bool auc_pending = false;
@@ -1062,8 +1070,9 @@ int dfb_predict(dfb_handle h, size_t nrows, const uint64_t* offset, const uint32
   b.nrows = nrows; b.offset = h->a_off.as<uint64_t>(); b.index = h->a_idx.as<uint32_t>();
   b.value = value ? h->a_val.as<float>() : nullptr;
   b.pred_io = h->a_pred.as<float>(); b.pred_acc = 1; b.V_dim = h->prm.V_dim; b.train = 0;
-  int nl = launch_fm(b, v, 1, s);
-  if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+  cudaError_t le = cudaSuccess;
+  int nl = launch_fm(b, v, 1, s, &le);
+  if (nl < 0) return fm_launch_fail(h, nl, le);
   h->launches += nl;
   DFB_CUDA(h, cudaMemcpyAsync(pred, h->a_pred.p, nrows * sizeof(float), cudaMemcpyDeviceToHost, s));
   DFB_CUDA(h, cudaStreamSynchronize(s));
@@ -1102,8 +1111,9 @@ int dfb_calc_grad(dfb_handle h, size_t nrows, const uint64_t* offset, const uint
   b.value = value ? h->a_val.as<float>() : nullptr; b.label = h->a_lab.as<float>();
   b.pred_in = h->a_pred.as<float>(); b.pred_io = nullptr; b.pred_acc = 0; b.V_dim = k; b.train = 1;
   b.prog = nullptr;
-  int nl = launch_fm(b, v, 1, s);
-  if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+  cudaError_t le = cudaSuccess;
+  int nl = launch_fm(b, v, 1, s, &le);
+  if (nl < 0) return fm_launch_fail(h, nl, le);
   h->launches += nl;
   if (k > 0)
     h->launches += launch_grad_finalize(k, npos, h->a_w.as<float>(), h->a_vpos.as<int>(), h->gxxp.as<float>(),
@@ -1659,8 +1669,9 @@ static int dev_fm_step_impl(dfb_handle h, size_t nrows, size_t nnz, const uint64
     b.occ_row = h->occ.as<uint32_t>(); b.occ_rowx = h->occ.as<unsigned long long>();
   }
   if (nrows) {
-    int nl = launch_fm(b, v, h->force_generic, s);
-    if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported FM configuration");
+    cudaError_t le = cudaSuccess;
+    int nl = launch_fm(b, v, h->force_generic, s, &le);
+    if (nl < 0) return fm_launch_fail(h, nl, le);
     h->launches += nl;
   }
   if (sorted) {

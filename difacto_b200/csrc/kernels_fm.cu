@@ -683,7 +683,17 @@ int launch_fm_raw(const FmBatch& b, const FmView& v, bool bf16_rows, cudaStream_
   });
 }
 
-int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s) {
+// dynamic shared memory above the default 48 KB per block needs the opt-in, and the limit counts the kernel's static
+// shared memory too (block_add_loss's 128 bytes): at V_dim 3072 the row of XV per warp is exactly 48 KB, and without
+// the opt-in the launch was refused
+template <typename Kern>
+void generic_smem_opt_in(Kern kern, size_t smem) {
+  cudaFuncAttributes fa;
+  if (cudaFuncGetAttributes(&fa, kern) == cudaSuccess && smem + fa.sharedSizeBytes > 48 * 1024)
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+}
+
+int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t s, cudaError_t* launch_err) {
   const int k = b.V_dim;
   bool fast = !force_generic && fm_fast_supported(k) &&
               v.v_pos != nullptr && aligned16(v.vbase) && (v.vstride % 4 == 0);
@@ -705,13 +715,18 @@ int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t
   size_t need = (b.nrows + 3) / 4;
   int grid = (int)(need < (size_t)(num_sms() * 16) ? (need ? need : 1) : (size_t)(num_sms() * 16));
   if (b.train) {
-    if (smem > 48 * 1024)
-      cudaFuncSetAttribute(k_fm_generic<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    generic_smem_opt_in(k_fm_generic<true>, smem);
     k_fm_generic<true><<<grid, threads, smem, s>>>(b, v);
   } else {
-    if (smem > 48 * 1024)
-      cudaFuncSetAttribute(k_fm_generic<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    generic_smem_opt_in(k_fm_generic<false>, smem);
     k_fm_generic<false><<<grid, threads, smem, s>>>(b, v);
+  }
+  // a launch the device refuses must fail the step, not leave it without a forward: its status, taken (and cleared)
+  // here, so that it fails this step and not the next
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) {
+    if (launch_err) *launch_err = e;
+    return kLaunchRefused;
   }
   return 1;
 }

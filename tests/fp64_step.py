@@ -23,7 +23,20 @@ Error bounds.  u = 2^-24 is the fp32 unit roundoff; 2^-50 is added to it for the
   * Forward, per row of n nonzeros: |pred - pred64| <= gamma(2n + k + 2) (sum |x w| + .5 (sum_f A_f^2 + Q)) with
     A_f = sum |x V_f| and Q = sum x^2 V_f^2: (XV)_f errs by gamma(n) A_f, its square by gamma(2n + 1) A_f^2, XXVV_f by
     gamma(n + 2) Q_f, their difference by one rounding more, the sum over f by gamma(k - 1), the final add by one.
-    The clamp is 1-Lipschitz.
+    The clamp is 1-Lipschitz.  This is order="sorted": the fast forward kernels form XXVV_f per f.
+  * order="generic" (k_fm_generic, kernels_fm.cu:457-554: every V_dim > 128, force_generic, the atomic scatter at
+    widths other than 8/16/32/64/128, and dfb_predict / dfb_calc_grad) forms the terms differently.  One warp per row,
+    lane l holds f = l, l + 32, ... (c = ceil(k / 32) of them):
+      - xv_f is a sequential sum over the row's n products a = fl(x V_f) (:498-499): errs by e_f = gamma(n) A_f;
+      - s1 = sum_f xv_f^2 is a per-lane fmaf chain over its c values, then a 5-level warp sum (:510-511).  Using xv_f
+        for XV_f errs by sum_f e_f (2 |XV_f| + e_f) (first order in e_f: far below gamma(2n + 1) A_f^2 when the x V_f
+        cancel), the sum itself by gamma(c + 5) of what it adds;
+      - acc2 = Q is a per-lane fmaf chain over all n c of the lane's a^2 (:500), then a 5-level warp sum (:512): a^2
+        errs by gamma(2), the chain and the tree by gamma(n c + 5) -- gamma(n c + 7) Q in all.  For n c > 2n + k that
+        is more than the sorted statement allows (n = 100 at k = 256; every row at k = 10000);
+      - s1 - acc2 and the final add with the linear part (a fmaf chain and a warp sum of n terms: gamma(n) sum |x w|)
+        round once each (:513); 0.5 (...) is exact.
+    Both forward bounds hold for every order their kernels use; neither is widened to cover the other.
   * |dp/dpred| = s (1 - s), s = sigmoid(pred), is at most 1/4 and falls with |pred|: over pred +- e_pred it is at most
     its value at max(0, |pred| - e_pred).  expf errs by 2 ulp (4u relative), the add and the division by u each:
     e_p = d + gamma(6) (|p| + d) with d = that slope times e_pred.  A row beyond +-20 by more than its bound is clamped
@@ -38,6 +51,9 @@ Error bounds.  u = 2^-24 is the fp32 unit roundoff; 2^-50 is added to it for the
     value, and its InitV flag may be either.  They are counted, and the count is capped.
   * The penalty's terms are non-negative and each is evaluated with at most 6 roundings; they are summed in fp32
     partials of at most `pen_partial(n_terms)` terms, then in double.
+  * Validation steps: the reference's Pull inserts every key of the batch (model_[key], sgd_updater.cc:32-56), so the
+    plugin calls (dfb_pull) do too; the fused entry points insert nothing on a validation step (a missing entry reads
+    as w = 0, no V row).  Reference(val_inserts=...) says which of the two a step is held to.
 
 Only tests import this module; it never imports the engine.
 """
@@ -188,6 +204,19 @@ def seg_sum(n, idx, t, et, mult=None):
     return v, e, a
 
 
+def generic_forward_bound(n, k, Lw, A, XV, S1, Q):
+    """the bound of k_fm_generic's prediction (module docstring, order="generic") for rows of n nonzeros (float64
+    tensor [B]), before the clamp: Lw = sum |x w|, A[B, k] = sum |x V_f|, XV[B, k], S1 = sum_f XV_f^2, Q"""
+    c = -(-k // 32)
+    e_f = gamma(n)[:, None] * A
+    e_sq = (e_f * (2 * XV.abs() + e_f)).sum(1)
+    e_s1 = e_sq + gamma(c + 5) * (S1 + e_sq)
+    e_Q = gamma(n * c + 7) * Q
+    e_d = e_s1 + e_Q + U * ((S1 - Q).abs() + e_s1 + e_Q)
+    e_lin = gamma(n) * Lw
+    return e_lin + 0.5 * e_d + U * (Lw + 0.5 * (S1 + Q) + e_lin + 0.5 * e_d) + ETA
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # the reference step
 # ---------------------------------------------------------------------------------------------------------------------
@@ -203,13 +232,16 @@ class Reference:
     """one SGD step from the pre-step state `pre` = (scal[U, 4] fea_cnt/w/sqrt_g/z, hasv[U] (-1 absent, 0, 1),
     V[U, k], cg[U, k]) of the batch's keys (batch_keys order), and the rng state `seed` before the step.
 
-    mode: "train", "val" (forward, loss, penalty, keys inserted) or "predict" (forward only).  mutant: one of MUTANTS,
-    a deliberately wrong variant used to show the comparison's sharpness.  hot_chunk: the chunk length of the hot-key
-    mutants."""
+    mode: "train", "val" (forward, loss, penalty; the batch's absent keys inserted when val_inserts) or "predict"
+    (forward only).  mutant: one of MUTANTS, a deliberately wrong variant used to show the comparison's sharpness.
+    hot_chunk: the chunk length of the hot-key mutants.  order: "sorted" or "generic", the forward kernel's summation
+    order (module docstring).  val_inserts: True for the reference and the plugin calls, False for the fused steps."""
 
     def __init__(self, batch, hp, pre, seed, push_cnt=False, mode="train", device="cpu", mutant=None, hot_chunk=256,
-                 budget=1 << 23):
+                 budget=1 << 23, order="sorted", val_inserts=True):
         assert mutant is None or mutant in MUTANTS, mutant
+        assert order in ("sorted", "generic"), order
+        self.order, self.val_inserts = order, bool(val_inserts)
         hp = dict(DEFAULTS, **hp)
         self.hp = {k: (float(np.float32(v)) if isinstance(v, float) else v) for k, v in hp.items()}
         self.k = k = int(hp["V_dim"])
@@ -239,7 +271,10 @@ class Reference:
         self.hv_pull = hv | self.push_initv
         Vp = np.where(hv[:, None], V, np.float32(0)).astype(np.float32) if k else np.zeros((Uk, 0), np.float32)
         if self.n_push:
-            Vp[self.push_initv] = initv_rows(self.seed0, 0, self.n_push, k, hp["V_init_scale"], device).cpu().numpy()
+            at, step = np.nonzero(self.push_initv)[0], max(1, budget // k)
+            for r0 in range(0, self.n_push, step):
+                Vp[at[r0:r0 + step]] = initv_rows(self.seed0, r0, len(at[r0:r0 + step]), k, hp["V_init_scale"],
+                                                  device).cpu().numpy()
         cgp = np.where(hv[:, None], cg, np.float32(0)).astype(np.float32) if k else Vp
         if mutant == "swap_tile_neighbour":        # a key's V row swapped with its successor's, mid-tile
             j = self._swap_index()
@@ -298,8 +333,12 @@ class Reference:
                 A[r0:r1].index_add_(0, seg, xV.abs())
                 Q[r0:r1].index_add_(0, seg, (xV * xV).sum(1))
         if k:
-            pred = lin + 0.5 * ((self.XV * self.XV).sum(1) - Q)
-            self.e_pred = gamma(2 * n + k + 2) * (Lw + 0.5 * ((A * A).sum(1) + Q)) + ETA
+            S1 = (self.XV * self.XV).sum(1)
+            pred = lin + 0.5 * (S1 - Q)
+            if self.order == "sorted":
+                self.e_pred = gamma(2 * n + k + 2) * (Lw + 0.5 * ((A * A).sum(1) + Q)) + ETA
+            else:
+                self.e_pred = generic_forward_bound(n, k, Lw, A, self.XV, S1, Q)
             if self.mutant != "no_clamp":     # 20 is an fp32 value: a row beyond it by more than its bound is exact
                 self.e_pred = torch.where(pred.abs() - self.e_pred >= 20, torch.zeros_like(pred), self.e_pred)
                 pred = pred.clamp(-20.0, 20.0)
@@ -497,6 +536,36 @@ def pen_partial_engine(n_keys, k):
     return max(32, -(-n_keys // 4096)) * (k + 1) + 5
 
 
+def _grid_warps(nwarps_needed, num_sms):
+    """the warps of a grid_warps(nwarps_needed, 8, num_sms * 8) launch of 256-thread blocks (kernels_table.cu:1160)"""
+    return min(max(1, -(-nwarps_needed // 8)), num_sms * 8) * 8
+
+
+def pen_partial_warp_per_key(num_sms):
+    """k_update_dense_generic (kernels_table.cu:326-369, launched at :1286) and k_penalty (:412-432, launched at
+    :1301): grid_warps(n, 8, num_sms * 8), one warp per key in a grid-stride loop.  Lane 0 adds pen_w and each lane
+    its ceil(k / 32) terms 0.5 V_l2 v^2 of every key its warp visits into one fp32 partial; then the warp sum (5 levels)
+    and a double atomic.  (pen_partial_engine bounds this too whenever num_sms >= 64; this is the launch's own count.)"""
+    def m(n_keys, k):
+        keys = -(-n_keys // _grid_warps(n_keys, num_sms))
+        return keys * (1 + -(-k // 32)) + 5
+    return m
+
+
+def pen_partial_update_fast(num_sms):
+    """k_update_fast<K> at the exact widths K = V_dim (kernels_table.cu:273-323, launched at :1281): G = 128 / K keys
+    per warp iteration, a group of K / 4 lanes per key; grid_warps(ceil(n / G), 8, num_sms * 8).  The group's first
+    lane adds pen_w, every lane adds 0.5 V_l2 (v.x^2 + v.y^2 + v.z^2 + v.w^2) -- four terms summed (3 adds) and scaled
+    (1 rounding) before they join the partial: at most 5 terms per key visited, each through at most 4 roundings
+    more, then the warp sum (5 levels) and a double atomic"""
+    def m(n_keys, k):
+        G = 128 // k
+        tiles = -(-n_keys // G)
+        it = -(-tiles // _grid_warps(tiles, num_sms))
+        return it * 5 + 4 + 5
+    return m
+
+
 def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC):
     """hold one step's result to the reference.  pre / post: the state of ref's keys before / after (read_entries
     layout); obs: dict with any of loss, penalty, auc, nrows, new_keys, new_vrows, n_keys_delta, n_vrows_delta,
@@ -531,7 +600,7 @@ def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC)
         if "auc" in obs and "label" in obs:
             R.exact("auc", np.float32(obs["auc"]) == np.float32(auc64(obs["label"], obs["pred"])),
                     f"{obs['auc']} vs float64 AUC of the returned predictions {auc64(obs['label'], obs['pred'])}")
-    inserted = ref.mode != "predict"
+    inserted = ref.mode == "train" or (ref.mode == "val" and ref.val_inserts)
     n_new_keys = int(ref.absent.sum()) if inserted else 0
     if "new_keys" in obs:
         R.exact("new_keys", obs["new_keys"] == n_new_keys, f"{obs['new_keys']} vs {n_new_keys}")
@@ -605,14 +674,18 @@ def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC)
         if "rng_after" in obs:
             want = int(lcg_jump(ref.seed0, 3 * k * n_new)[0])
             R.exact("rng", obs["rng_after"] == want, f"{obs['rng_after']} vs seed jumped by 3 V_dim {n_new} = {want}")
-        if len(upd):
-            Vw = initv_rows(ref.seed0, ref.n_push, len(upd), k, ref.hp["V_init_scale"], d).cpu().numpy()
+        badv, first = 0, ""
+        step = max(1, ref.budget // max(k, 1))          # the stream's rows in chunks of bounded size
+        for r0 in range(0, len(upd), step):
+            rows = upd[r0:r0 + step]
+            Vw = initv_rows(ref.seed0, ref.n_push + r0, len(rows), k, ref.hp["V_init_scale"], d).cpu().numpy()
             if ref.mutant == "adagrad_on_new_initv":
                 Vw = _adagrad_fresh(ref.hp, Vw)
-            badv = np.nonzero(~((V1[upd] == Vw).all(1) & (cg1[upd] == 0).all(1)))[0]
-            R.exact("InitV values", len(badv) == 0, f"{len(badv)} of {len(upd)} new rows differ from the stream, first "
-                    f"key {int(keys[upd[badv[0]]]):#018x}: {V1[upd[badv[0]]][:4]} vs {Vw[badv[0]][:4]}"
-                    if len(badv) else "")
+            bad = np.nonzero(~((V1[rows] == Vw).all(1) & (cg1[rows] == 0).all(1)))[0]
+            if len(bad) and not badv:
+                first = f"key {int(keys[rows[bad[0]]]):#018x}: {V1[rows[bad[0]]][:4]} vs {Vw[bad[0]][:4]}"
+            badv += len(bad)
+        R.exact("InitV values", badv == 0, f"{badv} of {len(upd)} new rows differ from the stream, first {first}")
     elif "rng_after" in obs:
         R.exact("rng", obs["rng_after"] == ref.seed0, "")
     return R

@@ -103,3 +103,118 @@ def test_every_mutant_rejects_the_oracle(mutant):
     F.check(ref(), pre, post, obs, what="true reference").assert_ok()
     R = F.check(ref(mutant), pre, post, obs, what=mutant)
     assert not R.ok(), f"{mutant} accepted: {R.summary()}"
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# k_fm_generic's summation order, emulated in float32
+# ---------------------------------------------------------------------------------------------------------------------
+def fmaf(a, b, c):
+    """fp32 fused multiply-add: a b of two fp32 values is exact in float64, so a b + c is rounded twice (float64,
+    then fp32).  The first rounding adds at most 2^-53 relative, within the 2^-50 that fp64_step.U allows beyond 2^-24"""
+    return (a.astype(np.float64) * b.astype(np.float64) + c.astype(np.float64)).astype(np.float32)
+
+
+def warp_sum(v):
+    """warp_sum (kernels_fm.cu:43-47) over the last axis (32 lanes): v += shfl_xor(v, o), o = 16 .. 1"""
+    lane = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        v = (v + v[..., lane ^ o]).astype(np.float32)
+    return v[..., 0]
+
+
+def emulate_generic_forward(off, x, w, V):
+    """the prediction k_fm_generic (kernels_fm.cu:469-515) computes for each row, in its order and fp32 roundings:
+    x, w per nonzero (float32 [nnz]), V[nnz, k] the nonzero's V row (zeros for a key without one, which the kernel skips:
+    adding 0 is exact either way)"""
+    B, k = len(off) - 1, V.shape[1]
+    c = -(-k // 32)
+    lens = np.diff(off.astype(np.int64))
+    nmax = int(lens.max())
+    chunks = -(-nmax // 32)
+    X = np.zeros((B, chunks * 32), np.float32)
+    W = np.zeros_like(X)
+    Vt = np.zeros((B, nmax, c * 32), np.float32)
+    for r in range(B):
+        a, b = int(off[r]), int(off[r + 1])
+        X[r, :b - a], W[r, :b - a] = x[a:b], w[a:b]
+        Vt[r, :b - a, :k] = V[a:b]
+    wsum = np.zeros((B, 32), np.float32)
+    for ch in range(chunks):                                     # lane l: nonzeros l, l + 32, ... (:473-489)
+        wsum = fmaf(X[:, ch * 32:(ch + 1) * 32], W[:, ch * 32:(ch + 1) * 32], wsum)
+    A = (X[:, :nmax, None] * Vt).astype(np.float32)             # a = x_t V_f (:498)
+    xv = np.zeros((B, c * 32), np.float32)
+    acc2 = np.zeros((B, 32), np.float32)
+    A4 = A.reshape(B, nmax, c, 32)
+    for t in range(nmax):
+        xv = (xv + A[:, t]).astype(np.float32)                  # xv[l] += a (:499)
+        for j in range(c):
+            acc2 = fmaf(A4[:, t, j], A4[:, t, j], acc2)          # acc2 = fmaf(a, a, acc2) (:500)
+    pred = warp_sum(wsum)                                        # pred = 0 + wsum (:505-507)
+    s1 = np.zeros((B, 32), np.float32)
+    xv4 = xv.reshape(B, c, 32)
+    for j in range(c):
+        s1 = fmaf(xv4[:, j], xv4[:, j], s1)                      # (:510)
+    d = (warp_sum(s1) - warp_sum(acc2)).astype(np.float32)
+    pred = (pred + np.float32(0.5) * d).astype(np.float32)     # (:513)
+    return np.clip(pred, np.float32(-20), np.float32(20))       # (:514)
+
+
+@pytest.mark.parametrize("V_dim", [129, 256, 3073, 10000])
+@pytest.mark.parametrize("valued", [False, True])
+def test_generic_order_emulation_within_generic_bound(V_dim, valued):
+    """random rows of up to 300 nonzeros, V rows of two scales (rows that stay inside +-20 and rows clamped), some keys
+    without a V row, some x = 0 and negative x"""
+    rng = np.random.default_rng(V_dim + valued)
+    lens = np.array([0, 1, 3, 17, 40, 100, 300, 300] + ([] if V_dim > 3072 else list(rng.integers(0, 300, 8))))
+    pool = np.unique(rng.integers(0, 1 << 40, 1200).astype(U64) * GOLDEN)
+    o, l, ids, v = csr(rng,lens, pool[rng.integers(0, len(pool), int(lens.sum()))], valued)
+    if valued:
+        v[rng.random(len(v)) < 0.05] = 0
+    keys, lidx, _ = F.batch_keys(ids)
+    Uk = len(keys)
+    scal = np.zeros((Uk, 4), np.float32)
+    scal[:, 1] = rng.normal(0, 0.3, Uk).astype(np.float32)
+    hasv = np.where(rng.random(Uk) < 0.9, 1, 0).astype(np.int32)
+    scale = np.where(rng.random(Uk) < 0.5, 0.02, 0.3)[:, None]
+    V = (rng.uniform(-1, 1, (Uk, V_dim)) * scale).astype(np.float32) * (hasv == 1)[:, None]
+    pre = (scal, hasv, V, np.zeros_like(V))
+    x = v if valued else np.ones(len(ids), np.float32)
+    emu = emulate_generic_forward(o, x, scal[lidx, 1], V[lidx])
+    ref = F.Reference((o, l, ids, v), dict(V_dim=V_dim), pre, 0, mode="predict", order="generic")
+    err = np.abs(emu.astype(np.float64) - ref.pred.numpy())
+    e = ref.e_pred.numpy()
+    assert (err <= e).all(), f"rows {np.nonzero(err > e)[0]}: error {err.max():.3g}, bound {e[np.argmax(err / e)]:.3g}"
+    assert (np.abs(ref.pred.numpy()) == 20).any() and (np.abs(ref.pred.numpy()) < 20).any()   # both kinds of rows
+    print(f"V_dim {V_dim} valued {valued}: max error / bound {float((err / np.where(e > 0, e, 1)).max()):.3g}")
+
+
+def csr(rng, lens, ids, valued):
+    off = np.concatenate([[0], np.cumsum(lens)]).astype(U64)
+    val = (rng.random(len(ids)).astype(np.float32) * 2 - 0.5) if valued else None
+    lab = np.where(rng.random(len(lens)) < 0.4, 1.0, -1.0).astype(np.float32)
+    return off, lab, ids, val
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# validation steps on ids the table never saw
+# ---------------------------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("val_inserts", [True, False])
+def test_validation_on_unseen_ids(val_inserts):
+    """the reference inserts a validation batch's absent keys (its Pull); the fused steps do not.  The oracle's step is
+    the first; the second is the same step with the state left as it was.  Each is accepted by the reference with the
+    matching val_inserts and rejected by the other"""
+    rng = np.random.default_rng(41)
+    hp = hyper(8, 0)
+    M = O.Oracle(**hp)
+    pool = np.unique(rng.integers(0, 1 << 40, 600).astype(U64) * GOLDEN)
+    for _ in range(2):
+        o, l, i, v = rand_batch(rng, pool[:300], 80, False)
+        M.sgd_step(o, i, v, l, push_cnt=True)
+    b = rand_batch(rng, pool, 80, True)                     # half of the ids unseen
+    ref, pre, post, obs = oracle_step(M, hp, b, False, "val")
+    assert (pre[1] < 0).sum() > 20 and obs["n_keys_delta"] == (pre[1] < 0).sum()
+    if not val_inserts:
+        post, obs = pre, dict(obs, n_keys_delta=0)
+    F.check(F.Reference(b, hp, pre, M.seed(), False, "val", val_inserts=val_inserts), pre, post, obs).assert_ok()
+    R = F.check(F.Reference(b, hp, pre, M.seed(), False, "val", val_inserts=not val_inserts), pre, post, obs)
+    assert not R.ok(), R.summary()

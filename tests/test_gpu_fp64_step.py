@@ -89,7 +89,7 @@ class Run:
                    rng_after=E.rng_state(), pred=pred, auc=pr.auc, label=l)
         mode = {"train_dev": "train", "train_pred": "train"}.get(kind, kind)
         t0 = time.perf_counter()
-        ref = F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", hot_chunk=self.hot_chunk)
+        ref = F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", hot_chunk=self.hot_chunk, val_inserts=False)
         R = F.check(ref, pre, post, obs, what=f"{kind} push={push}", pen_partial=F.pen_partial_engine,
                     amb_frac=self.amb_frac)
         t_ref = time.perf_counter() - t0
@@ -97,7 +97,8 @@ class Run:
         R.assert_ok()
         F.assert_unchanged(out_pre, E.read_entries(out), out, f"{kind} push={push}")
         for m in mutants:
-            Rm = F.check(F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", mutant=m, hot_chunk=self.hot_chunk),
+            Rm = F.check(F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", mutant=m, hot_chunk=self.hot_chunk,
+                                     val_inserts=False),
                          pre, post, obs, what=m, pen_partial=F.pen_partial_engine)
             assert not Rm.ok(), f"the {m} variant of the reference accepts the engine's step: {Rm.summary()}"
         if mode != "predict":
