@@ -215,7 +215,9 @@ class Engine:
     capacities; with table_capacity_max / V_capacity_max above them the table and the V-row pool grow on demand, and
     table_stats() reports the current capacities; shard_growth=1 lets such an engine be a rank of the fused sharded
     store, whose owners then grow by the keys they receive.  score_only=True (optionally V_storage="bf16") makes a scoring-only
-    engine: restore and predict_raw* only, V rows without their AdaGrad halves; what it refuses raises DfbError."""
+    engine: restore and predict_raw* only, V rows without their AdaGrad halves; what it refuses raises DfbError.  It may
+    also be a rank of a fused sharded store of two or more ranks (shard_init), which then runs shard_predict_async /
+    shard_begin_predict_async only."""
 
     def __init__(self, **kwargs):
         L = lib()

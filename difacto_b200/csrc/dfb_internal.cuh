@@ -234,8 +234,9 @@ int launch_fm(const FmBatch& b, const FmView& v, int force_generic, cudaStream_t
 // bf16_rows (predict only; a scoring-only engine with V_storage = bf16): v.vbase points at bf16 elements and vstride
 // counts them; each lane widens its 4 columns to fp32 and everything after the load is the fp32 kernels' code
 int launch_fm_raw(const FmBatch& b, const FmView& v, bool bf16_rows, cudaStream_t s);
-// MODE 3: partial interaction sums of every source's rows (see PartArgs); v.vbase/vstride = the table rows
-int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s);
+// MODE 3: partial interaction sums of every source's rows (see PartArgs); v.vbase/vstride = the table rows.
+// bf16_rows: a scoring-only owner's bf16 V rows, widened in the row load as in launch_fm_raw
+int launch_fm_partial(int V_dim, bool valued, bool bf16_rows, const FmView& v, const PartArgs& pa, cudaStream_t s);
 int launch_grad_finalize(int V_dim, size_t nkeys, const float* weights, const int* V_pos,
                          const float* xxp, float* grad, cudaStream_t s);
 

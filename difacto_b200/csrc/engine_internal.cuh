@@ -141,11 +141,12 @@ struct dfb_engine {
     return !force_generic && dfb::fm_fast_supported(prm.V_dim) && (!is_train || scatter_sorted);
   }
   int fail(int code, const std::string& msg) { err = msg; return code; }
-  // at the top of every entry point that trains, counts features, reads or writes rows, saves, prunes or shards: a
+  // at the top of every entry point that trains, counts features, validates, reads or writes rows, saves or prunes: a
   // scoring-only engine holds neither the AdaGrad half of a row nor, with bf16 rows, the V values a snapshot stores
   int refuse_score_only(const char* call) {
     return fail(DFB_ERR_INVALID, std::string(call) + " is not available on a score_only = 1 engine (it restores a "
-                                 "model and scores with dfb_predict_raw_*)");
+                                 "model and scores with dfb_predict_raw_*, or as a rank of the sharded store with "
+                                 "dfb_shard_*predict_async)");
   }
   int cuda_fail(cudaError_t e, const char* what) {
     err = std::string(what) + ": " + cudaGetErrorString(e);

@@ -117,7 +117,7 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 // MODE 2: training, "emit": writes p_i, p_i*XV_i and the (row[,x]) payload of every nnz so that
 //         the gradient can be reduced per key without atomics (kernels_table.cu: k_bwd_update).
 // MODE 3: owner side of the fused sharded store: partial sums of every worker's rows over this owner's
-//         key segment, stored into the workers' mailboxes (see PartArgs).
+//         key segment, stored into the workers' mailboxes (see PartArgs).  BF16 here: a scoring-only owner's rows.
 // RAW (MODE 0 and 2): the nonzeros carry raw feature ids (b.ids); the metadata of each is probed in the table
 //         (probe_raw) instead of being read from a pulled view through a localized index.  Everything after the
 //         metadata is the same code, so the predictions (and p, p*XV) are bit-identical to those of the steps that
@@ -137,7 +137,7 @@ __device__ __forceinline__ void block_add_loss(float loss_acc, size_t nrows, Dev
 template <int K, int MODE, bool HAS_VAL, bool PAD = false, bool RAW = false, bool BF16 = false>
 __global__ void __launch_bounds__(256, K == 32 ? DFB_FM_MINBLOCKS32 : DFB_FM_MINBLOCKS) k_fm_fast(FmBatch b, FmView v, PartArgs pa) {
   constexpr bool TRAIN = MODE == 1;
-  static_assert(!BF16 || (RAW && MODE == 0), "bf16 rows: the raw-id predict step only");
+  static_assert(!BF16 || (RAW && MODE == 0) || MODE == 3, "bf16 rows: the raw-id predict step and the owner's partial sums only");
   static_assert(!(PAD && TRAIN), "the atomic scatter runs the exact widths only");
   static_assert(!RAW || MODE == 0 || MODE == 2, "raw ids: predict and emit only");
   constexpr int LPR = K / 4;                 // lanes per V row, one float4 each
@@ -643,7 +643,8 @@ int launch_fast_k(const FmBatch& b, const FmView& v, cudaStream_t s) {
   return 1;
 }
 
-template <int K, bool PAD>
+// BF16: the owner is a scoring-only engine with bf16 V rows (the same kernel but for the row load)
+template <int K, bool PAD, bool BF16>
 int launch_partial_k(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s) {
   FmBatch b;
   memset(&b, 0, sizeof(b));
@@ -651,10 +652,10 @@ int launch_partial_k(int V_dim, bool valued, const FmView& v, const PartArgs& pa
   const int grid = num_sms() * 8;
   if constexpr (PAD) {
     if (!valued) return -1;       // the owners' wire format is always valued (kernels_shard.cu)
-    k_fm_fast<K, 3, true, true><<<grid, 256, 0, s>>>(b, v, pa);
+    k_fm_fast<K, 3, true, true, false, BF16><<<grid, 256, 0, s>>>(b, v, pa);
   } else {
-    if (valued) k_fm_fast<K, 3, true><<<grid, 256, 0, s>>>(b, v, pa);
-    else        k_fm_fast<K, 3, false><<<grid, 256, 0, s>>>(b, v, pa);
+    if (valued) k_fm_fast<K, 3, true, false, false, BF16><<<grid, 256, 0, s>>>(b, v, pa);
+    else        k_fm_fast<K, 3, false, false, false, BF16><<<grid, 256, 0, s>>>(b, v, pa);
   }
   return 1;
 }
@@ -663,11 +664,14 @@ int launch_partial_k(int V_dim, bool valued, const FmView& v, const PartArgs& pa
 
 bool fm_fast_supported(int k) { return fast_lane_width(k) != 0; }
 
-int launch_fm_partial(int V_dim, bool valued, const FmView& v, const PartArgs& pa, cudaStream_t s) {
+int launch_fm_partial(int V_dim, bool valued, bool bf16_rows, const FmView& v, const PartArgs& pa, cudaStream_t s) {
   return with_lane_width(V_dim, [&](auto kc) {
     constexpr int K = decltype(kc)::value;
-    return V_dim == K ? launch_partial_k<K, false>(V_dim, valued, v, pa, s)
-                      : launch_partial_k<K, true>(V_dim, valued, v, pa, s);
+    if (bf16_rows)
+      return V_dim == K ? launch_partial_k<K, false, true>(V_dim, valued, v, pa, s)
+                        : launch_partial_k<K, true, true>(V_dim, valued, v, pa, s);
+    return V_dim == K ? launch_partial_k<K, false, false>(V_dim, valued, v, pa, s)
+                      : launch_partial_k<K, true, false>(V_dim, valued, v, pa, s);
   });
 }
 

@@ -267,7 +267,7 @@ int shard_phase(dfb_engine* h, int phase) {
     FmView v;
     memset(&v, 0, sizeof(v));
     v.vbase = h->tab.V; v.vstride = h->tab.rs; v.l2hint = h->l2_hints; v.wv_last = h->l2_hints;
-    int nl = launch_fm_partial(K, true, v, pa, O);
+    int nl = launch_fm_partial(K, true, h->tab.vonly == 2, v, pa, O);
     if (nl < 0) return h->fail(DFB_ERR_INVALID, "unsupported V_dim for the sharded store");
     h->launches += nl;
   }
@@ -451,18 +451,23 @@ extern "C" {
 int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t max_nnz, size_t seg_keys,
                    size_t seg_nnz, size_t* mailbox_bytes) {
   if (!h) return DFB_ERR_INVALID;
-  DFB_NOT_SCORE_ONLY(h, "dfb_shard_init");
   if (h->shard) return h->fail(DFB_ERR_INVALID, "dfb_shard_init was already called");
   if (nranks < 1 || nranks > 8 || rank < 0 || rank >= nranks) return h->fail(DFB_ERR_INVALID, "1 <= nranks <= 8, 0 <= rank < nranks");
   if (max_rows == 0 || max_nnz == 0 || max_nnz > 0x7fffffffULL || max_rows > 0x7fffffffULL)
     return h->fail(DFB_ERR_INVALID, "max_rows / max_nnz out of range");
+  // a scoring engine on its own already scores its whole model with dfb_predict_raw_*: a one-rank store would only add
+  // the store's workspaces
+  if (h->score_only && nranks < 2)
+    return h->fail(DFB_ERR_INVALID, "dfb_shard_init: a score_only = 1 engine is a rank of a store of nranks >= 2 (on "
+                                    "its own it scores with dfb_predict_raw_*)");
   const int ks = h->tab.ks;
   if (!h->sorted_path())
     return h->fail(DFB_ERR_INVALID, "the fused sharded store needs V_dim in 0..128, scatter=sorted and no force_generic "
                                     "(other configurations: the all_to_all ShardedStore)");
   // a growing rank bounds each step's insertions by the keys its owner received, counted on the device
-  // (shard_growth = 1, growth.cu); without that opt-in the store keeps fixed capacities
-  if (h->grow.on && !h->shard_growth)
+  // (shard_growth = 1, growth.cu); without that opt-in the store keeps fixed capacities.  A scoring rank's predict
+  // steps never insert: it grows only in dfb_restore*, which runs between steps.
+  if (h->grow.on && !h->shard_growth && !h->score_only)
     return h->fail(DFB_ERR_INVALID, "the fused sharded store does not grow its shards: create the engine with "
                                     "table_capacity_max = table_capacity and V_capacity_max = V_capacity, or with "
                                     "shard_growth = 1");
@@ -495,13 +500,18 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
       if ((e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
   if ((e = cudaEventCreateWithFlags(&sh->ev_grow, cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
   const size_t tot = (size_t)nranks * Kseg;
+  // a scoring rank (score_only = 1) runs predict steps only: it has no InitV requests (flags, ws), no pull-time V rows
+  // to save for the updates (conf, vsave) and no hot keys to pre-reduce.  Its mailbox is a training rank's: the peers
+  // address it without knowing which kind it is.
+  const bool train = !h->score_only;
   int rc = 0;
   if ((rc = h->ensure(sh->wb, 2 * sizeof(ShardBounds))) || (rc = h->ensure(sh->slot[0], tot * 4)) || (rc = h->ensure(sh->slot[1], tot * 4)) || (rc = h->ensure(sh->w, tot * 4)) ||
-      (rc = h->ensure(sh->vrow, tot * 4)) || (rc = h->ensure(sh->wv, tot * 8)) || (rc = h->ensure(sh->flags, tot * 4)) ||
-      (rc = h->ensure(sh->ws, (tot / 32 + 64) * 4)))
+      (rc = h->ensure(sh->vrow, tot * 4)) || (rc = h->ensure(sh->wv, tot * 8)))
     return fail(rc);
-  if (nranks > 1 && ((rc = h->ensure(sh->conf[0], tot)) || (rc = h->ensure(sh->conf[1], tot)) ||
-                     (rc = h->ensure(sh->vsave, tot * (size_t)ks * 4))))
+  if (train && ((rc = h->ensure(sh->flags, tot * 4)) || (rc = h->ensure(sh->ws, (tot / 32 + 64) * 4))))
+    return fail(rc);
+  if (train && nranks > 1 && ((rc = h->ensure(sh->conf[0], tot)) || (rc = h->ensure(sh->conf[1], tot)) ||
+                              (rc = h->ensure(sh->vsave, tot * (size_t)ks * 4))))
     return fail(rc);
   // Every workspace a step can touch is allocated NOW, for the declared capacities: a cudaMalloc / cudaFree in the
   // middle of a step is not just slow -- with peer access enabled it synchronises the peer devices, whose pollers
@@ -517,7 +527,7 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
         (rc = h->ensure(h->l_tmp, localize_sort_tmp_bytes(n1))) || (rc = h->ensure(sh->rowcnt, (size_t)nranks * (B + 1) * 4)) ||
         (rc = h->ensure(sh->pred[0], B * 4)) || (rc = h->ensure(sh->pred[1], B * 4)) || (rc = h->ensure(h->auc_k, B * 4)) ||
         (rc = h->ensure(h->auc_v, B * 4)) || (rc = h->ensure(h->auc_tmp, sort_tmp_bytes(B))) ||
-        (rc = dfbh::hot_ws(h, Kseg, Nseg, &hws)))
+        (train && (rc = dfbh::hot_ws(h, Kseg, Nseg, &hws))))
       return fail(rc);
     for (auto& in : h->in)
       if ((rc = h->ensure(in.off, (B + 1) * 8)) || (rc = h->ensure(in.ids, n1 * 8)) || (rc = h->ensure(in.val, n1 * 4)) ||
@@ -575,6 +585,7 @@ int dfb_shard_connect(dfb_handle h, void* const* peer_mailbox) {
 int dfb_shard_step_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
                        const float* d_value_or_null, const float* d_label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_shard_step_dev");
   DFB_CUDA(h, cudaSetDevice(h->device));
   return shard_step(h, nrows, nnz, d_offset, d_ids, d_value_or_null, d_label, push_cnt, is_train, nullptr, nullptr);
 }
@@ -582,6 +593,7 @@ int dfb_shard_step_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d
 int dfb_shard_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
                          const float* label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_shard_step_async");
   DFB_TRY(dfbh::check_csr(h, nrows, offset));
   if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
   DFB_CUDA(h, cudaSetDevice(h->device));
@@ -599,6 +611,7 @@ int dfb_shard_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, con
 int dfb_shard_begin_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset, const uint64_t* d_ids,
                         const float* d_value_or_null, const float* d_label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_shard_begin_dev");
   DFB_CUDA(h, cudaSetDevice(h->device));
   return shard_begin(h, nrows, nnz, d_offset, d_ids, d_value_or_null, d_label, push_cnt, is_train, nullptr, nullptr);
 }
@@ -606,6 +619,7 @@ int dfb_shard_begin_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* 
 int dfb_shard_begin_async(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
                           const float* label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
+  DFB_NOT_SCORE_ONLY(h, "dfb_shard_begin_async");
   DFB_TRY(dfbh::check_csr(h, nrows, offset));
   if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
   DFB_CUDA(h, cudaSetDevice(h->device));

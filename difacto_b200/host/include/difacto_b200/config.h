@@ -83,7 +83,9 @@ struct SGDLearnerParam {
   std::string data_in, data_val, data_format = "libsvm", model_out, model_in, loss = "fm";
   std::string pred_out;   // engine-only: where task=predict writes one prediction per input row
                           // (task=predict also takes the engine keys score_only = 1 and V_storage = bf16: the model
-                          // is loaded without its AdaGrad state, V rows in fp32 or bf16; num_gpus = 1 only)
+                          // is loaded without its AdaGrad state, V rows in fp32 or bf16, on one GPU or -- the parts of
+                          // a num_gpus run, num_gpus = N -- into N scoring ranks of the sharded store, which run predict
+                          // steps with or without pred_out)
   int max_num_epochs = 20, num_jobs_per_epoch = 10, batch_size = -1, shuffle = 10;
   float neg_sampling = 1, stop_rel_objv = 1e-5f, stop_val_auc = 1e-5f;
   int fused = 1;   // engine-only: 1 = raw block -> one device call, 2 = host localizer + one device call,

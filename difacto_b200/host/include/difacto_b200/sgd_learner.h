@@ -82,8 +82,10 @@ class SGDLearner : public Learner {
   void RunEpoch(int epoch, int job_type, sgd::Progress* prog);
   void IterateData(const sgd::Job& job, sgd::Progress* prog);
   /** num_gpus > 1: one epoch over all N * num_jobs_per_epoch file parts, part i handled by worker i % N.
-   * pred_out (task=predict): predict steps, and the predictions of every row to that file, in file order */
-  void RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, const std::string* pred_out = nullptr);
+   * predict (task=predict): predict steps instead of validation steps (penalty 0); pred_out: the predictions of every
+   * row to that file, in file order */
+  void RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, bool predict = false,
+                       const std::string* pred_out = nullptr);
   /** the model X (one file) or X_part-0 .. of a num_gpus = M run into the engines (model_in, checkpoint_in) */
   void LoadShards(const std::string& base);
   /** checkpoint_in: the model, the id ranges and the position in the run of the checkpoint the pointer file names */
@@ -112,6 +114,7 @@ class SGDLearner : public Learner {
   SGDLearnerParam param_;
   std::vector<EpochCallback> epoch_end_callback_;
   std::vector<std::shared_ptr<GpuEngine>> shard_engines_;     // GPUs 1..N-1 (num_gpus > 1)
+  bool score_only_ = false;     // the engine key score_only = 1: scoring-only engines, which run predict steps only
 
   // checkpoints: the settings the state record fingerprints, the run's position (kept current by the drivers), the
   // state to resume from, and the write in flight

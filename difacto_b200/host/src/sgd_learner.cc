@@ -44,6 +44,7 @@ std::string FloatSetting(const std::string& v) {
   if (v.empty() || *end) return v;
   return FloatSetting(f);
 }
+bool FileExists(const std::string& fn) { return static_cast<bool>(std::ifstream(fn, std::ios::binary)); }
 std::string IntSetting(const std::string& v) {
   char* end = nullptr;
   const long long x = strtoll(v.c_str(), &end, 10);
@@ -83,12 +84,15 @@ std::vector<std::pair<std::string, std::string>> SGDLearner::Settings(const SGDL
 // SGDLearner::Init, sgd_learner.cc:229-246
 KWArgs SGDLearner::Init(const KWArgs& kwargs) {
   KWArgs remain = param_.InitAllowUnknown(kwargs);
-  // score_only / V_storage are engine keys and reach dfb_create with the rest; the sharded store keeps the training
-  // layout in its shards, so a scoring-only model is scored on one GPU
-  if (param_.num_gpus > 1)
-    for (const auto& kv : kwargs)
-      if (kv.first == "score_only" && kv.second != "0")
-        throw ParamError("score_only = 1 needs num_gpus = 1 (the sharded predict keeps training-layout shards)");
+  // score_only / V_storage are engine keys and reach dfb_create with the rest (every GPU's engine: with num_gpus > 1
+  // each rank of the sharded store holds its shard in V-only rows)
+  for (const auto& kv : kwargs)
+    if (kv.first == "score_only") score_only_ = kv.second != "0";
+  // N scoring GPUs load the parts of a model a num_gpus run saved.  A one-file model was trained on one GPU, so its
+  // scoring-only layout (half or a quarter of the rows) fits one GPU: it is scored there, without the store's workspaces
+  if (score_only_ && param_.num_gpus > 1 && !FileExists(param_.model_in + "_part-0"))
+    throw ParamError("score_only = 1 with num_gpus > 1 scores the parts of a model saved by a num_gpus run (model_in = X "
+                     "reads X_part-0 ...); score a one-file model with num_gpus = 1");
   settings_ = Settings(param_, kwargs);
   auto* updater = new GpuSGDUpdater();
   std::shared_ptr<Updater> holder(updater);
@@ -129,8 +133,6 @@ KWArgs SGDLearner::Init(const KWArgs& kwargs) {
 }
 
 namespace {
-bool FileExists(const std::string& fn) { return static_cast<bool>(std::ifstream(fn, std::ios::binary)); }
-
 // ps-lite's key range of shard r of S (postoffice.cc:127-136; the tail above UINT64_MAX/S*S belongs to S-1), as
 // an inclusive [lo, hi]
 void KeyRange(uint32_t r, uint32_t S, uint64_t* lo, uint64_t* hi) {
@@ -242,7 +244,10 @@ sgd::Progress SGDLearner::Predict() {
     LoadShards(param_.model_in);
     sgd::Progress prog;
     param_.data_val = param_.data_in;
-    RunEpochSharded(0, sgd::Job::kValidation, &prog, param_.pred_out.empty() ? nullptr : &param_.pred_out);
+    // a scoring-only store runs predict steps only (its ranks refuse validation steps); a training-layout one predicts
+    // when it writes the predictions, and otherwise validates (Progress with the penalty)
+    const bool write = !param_.pred_out.empty();
+    RunEpochSharded(0, sgd::Job::kValidation, &prog, write || score_only_, write ? &param_.pred_out : nullptr);
     if (verbose) printf(" - Prediction: %s, rows = %g\n", prog.TextString().c_str(), prog.nrows);
     return prog;
   }
@@ -373,15 +378,15 @@ void SGDLearner::RunEpoch(int epoch, int job_type, sgd::Progress* prog) {
 //
 // pred_out: the rows of part i go to a temporary file <pred_out>.part-<i> (host memory stays bounded), which are
 // concatenated in part order into pred_out at the end and removed.
-void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, const std::string* pred_out) {
+void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, bool predict, const std::string* pred_out) {
   const int N = param_.num_gpus;
   const int nparts = N * param_.num_jobs_per_epoch;
   const bool train = job_type == sgd::Job::kTraining;
   const bool push_cnt = train && epoch == 0;      // sgd_learner.cc:201-202
-  const bool predict = pred_out != nullptr;
+  const bool write = pred_out != nullptr;
   auto tmp_name = [&](int part) { return *pred_out + ".part-" + std::to_string(part); };
-  std::vector<FILE*> part_files(predict ? nparts : 0, nullptr);
-  std::vector<PinnedBuf> pred_bufs(predict ? N : 0);
+  std::vector<FILE*> part_files(write ? nparts : 0, nullptr);
+  std::vector<PinnedBuf> pred_bufs(write ? N : 0);
   std::vector<int> step_part(N, -1);
   auto close_parts = [&]() {
     for (auto& f : part_files) if (f) { fclose(f); f = nullptr; }
@@ -443,7 +448,7 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
       const uint64_t* off = blk.size ? reinterpret_cast<const uint64_t*>(blk.offset) : nullptr;
       if (predict) {       // every rank predicts in the same step (the step is collective)
         eng->Check(dfb_shard_begin_predict_async(eng->handle(), blk.size, off, blk.index, blk.value, blk.label,
-                                                 pred_bufs[r].get<real_t>(blk.size ? blk.size : 1)),
+                                                 write ? pred_bufs[r].get<real_t>(blk.size ? blk.size : 1) : nullptr),
                    "dfb_shard_begin_predict_async");
       } else {
         eng->Check(dfb_shard_begin_async(eng->handle(), blk.size, off, blk.index, blk.value, blk.label, push_cnt ? 1 : 0,
@@ -456,7 +461,7 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
       dfb_progress pr;
       ShardEngine(r)->Check(dfb_wait_step(ShardEngine(r)->handle(), &pr), "dfb_wait_step");
       prog->loss += pr.loss; prog->penalty += pr.penalty; prog->auc += pr.auc; prog->nrows += pr.nrows;
-      if (predict && step_part[r] >= 0) {
+      if (write && step_part[r] >= 0) {
         FILE*& f = part_files[step_part[r]];
         if (!f && !(f = fopen(tmp_name(step_part[r]).c_str(), "w"))) {
           close_parts();
@@ -477,7 +482,7 @@ void SGDLearner::RunEpochSharded(int epoch, int job_type, sgd::Progress* prog, c
       epoch_prog_ = nullptr;
     }
   }
-  if (!predict) return;
+  if (!write) return;
   close_parts();
   FILE* fo = fopen(pred_out->c_str(), "w");
   if (!fo) throw Error("failed to open pred_out " + *pred_out);

@@ -126,11 +126,13 @@ typedef struct {
  *                         a restore grows the engine up to the maxima).  has_aux reads 0.  Also allowed:
  *                         dfb_table_stats, dfb_row_bytes, dfb_id_range_get/set, dfb_sync, dfb_prefetch_raw, the
  *                         Progress reads (dfb_wait_step, dfb_read_progress), dfb_evaluate / dfb_auc, the timing
- *                         calls, dfb_destroy.  Every call that trains, counts features, validates, reads or writes
- *                         rows, saves, prunes or shards returns DFB_ERR_INVALID with a message naming score_only
+ *                         calls, dfb_destroy.  It may be a scoring rank of the fused sharded store (dfb_shard_init;
+ *                         its predict steps, see there).  Every call that trains, counts features, validates, reads
+ *                         or writes rows, saves or prunes returns DFB_ERR_INVALID with a message naming score_only
  *                         and changes nothing: dfb_train_step*, dfb_train_step_raw*, dfb_push_feacnt, dfb_pull,
  *                         dfb_push_grad, dfb_predict, dfb_calc_grad, dfb_read_entries, dfb_dev_*, dfb_snapshot*,
- *                         dfb_prune, dfb_shard_init.  Needs 0 <= V_dim <= 128 and force_generic = 0 (DFB_ERR_PARAM
+ *                         dfb_prune, dfb_shard_step_*, dfb_shard_begin_dev / _async.  Needs 0 <= V_dim <= 128 and
+ *                         force_generic = 0 (DFB_ERR_PARAM
  *                         otherwise): the predict step of other configurations is the validation step.
  *                         The fp32 scoring engine's predictions and Progress are bit-identical to the training
  *                         engine's predict step on the same model.
@@ -477,8 +479,17 @@ int dfb_dev_fm_step_peer(dfb_handle h, size_t nrows, size_t nnz, const uint64_t*
  * per-example partial interaction sums (see csrc/kernels_shard.cu); nothing is synchronised with the host.
  *   dfb_shard_init     allocate this rank's mailbox (capacity: max_rows x max_nnz per minibatch; seg_keys /
  *                      seg_nnz = capacity of one (worker, owner) key segment, 0 = twice the even share).  Needs
- *                      0 <= V_dim <= 128, scatter=sorted and force_generic=0 (DFB_ERR_INVALID otherwise); a
- *                      score_only = 1 engine is refused (the shards keep the training layout)
+ *                      0 <= V_dim <= 128, scatter=sorted and force_generic=0 (DFB_ERR_INVALID otherwise).
+ *                      A score_only = 1 engine becomes a scoring rank of a store of nranks >= 2 (nranks = 1:
+ *                      DFB_ERR_INVALID naming score_only; alone it scores with dfb_predict_raw_*): its shard is
+ *                      V-only rows (fp32 or bf16), it allocates none of the training steps' workspaces (pull-time V rows of shared keys, InitV
+ *                      flags, hot-key pre-reduction), and it may grow (up to its maxima, in dfb_restore* only: its
+ *                      steps never insert) without shard_growth.  It runs dfb_shard_predict_async and
+ *                      dfb_shard_begin_predict_async; dfb_shard_step_* and dfb_shard_begin_dev / _async (training,
+ *                      feature counts or validation) return DFB_ERR_INVALID naming score_only before anything is
+ *                      enqueued.  Its mailbox is a training rank's (same mailbox_bytes), so one store may mix training
+ *                      and scoring ranks for predict steps; fp32 scoring ranks predict bit-identically to training
+ *                      ranks holding the same model
  *   dfb_shard_export   the mailbox pointer (peers in the same process) and its CUDA IPC handle (peers in
  *                      other processes open it with dfb_peer_open)
  *   dfb_shard_connect  the peers' mailbox pointers, indexed by rank (entry [rank] is ignored)
