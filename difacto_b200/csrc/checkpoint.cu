@@ -94,27 +94,16 @@ struct Scratch {
 // the writer's two pinned chunks and their events: a call's own (dfb_snapshot_write), or kept by a frozen copy
 // across its writes and freed at its release, off the writer thread
 struct PinnedChunks {
-  char* pin[2] = {nullptr, nullptr};
-  cudaEvent_t ev[2] = {nullptr, nullptr};
+  PinnedHost<char> pin[2];
+  Event ev[2];
   size_t bytes = 0;
-  PinnedChunks() = default;
-  PinnedChunks(const PinnedChunks&) = delete;
-  PinnedChunks& operator=(const PinnedChunks&) = delete;
-  ~PinnedChunks() { release(); }
-  void release() {
-    for (int i = 0; i < 2; ++i) {
-      if (pin[i]) cudaFreeHost(pin[i]);
-      if (ev[i]) cudaEventDestroy(ev[i]);
-      pin[i] = nullptr; ev[i] = nullptr;
-    }
-    bytes = 0;
-  }
   int ensure(ErrSink* es, size_t chunk) {
     if (chunk <= bytes) return 0;
-    release();
+    bytes = 0;
+    for (auto& p : pin) p.reset();      // both before the larger ones are allocated
     for (int i = 0; i < 2; ++i) {
-      DFB_CUDA(es, cudaHostAlloc(reinterpret_cast<void**>(&pin[i]), chunk, cudaHostAllocDefault));
-      DFB_CUDA(es, cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming));
+      DFB_CUDA(es, pin[i].alloc(chunk));
+      DFB_CUDA(es, ev[i].create());
     }
     bytes = chunk;
     return 0;
@@ -194,8 +183,8 @@ int write_records(const Table& t, const TableState& st, int k, bool aux, size_t 
   DFB_TRY(sc.dalloc(&ws.tmp, ws.tmp_bytes));
   DFB_TRY(sc.dalloc(&ws.out, max_bytes));
   DFB_TRY(pc.ensure(es, chunk));
-  char* const* pin = pc.pin;
-  const cudaEvent_t* ev = pc.ev;
+  const PinnedHost<char>* pin = pc.pin;
+  const Event* ev = pc.ev;
   for (const Pass& p : passes) {
     const int nl = launch_ckpt_pass(t, p.b0, p.b1, p.nk, aux, k, ws, s);
     if (nl < 0) return es->fail(DFB_ERR_CUDA, "snapshot pass failed (radix sort / scan)");

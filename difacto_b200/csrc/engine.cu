@@ -30,11 +30,9 @@ int dfb_engine::ensure(DevBuf& b, size_t bytes) {
     if ((e = cudaStreamSynchronize(copy_stream)) != cudaSuccess) return cuda_fail(e, "sync");
     if (loc_stream && (e = cudaStreamSynchronize(loc_stream)) != cudaSuccess) return cuda_fail(e, "sync");
     if (shard) dfbh::shard_sync(this);
-    cudaFree(b.p);
-    b.p = nullptr; b.bytes = 0;
+    b.reset();
   }
-  if ((e = cudaMalloc(&b.p, want)) != cudaSuccess) return cuda_fail(e, "cudaMalloc(workspace)");
-  b.bytes = want;
+  if ((e = b.alloc(want)) != cudaSuccess) return cuda_fail(e, "cudaMalloc(workspace)");
   return 0;
 }
 
@@ -188,7 +186,7 @@ int dfbh::prof_drain(dfb_engine* h) {
       char& used = h->pev_used[r * dfb_engine::kStages + st];
       if (!used) continue;
       float ms = 0.f;
-      cudaEvent_t* e = &h->pev[(r * dfb_engine::kStages + st) * 2];
+      const Event* e = &h->pev[(r * dfb_engine::kStages + st) * 2];
       if (cudaEventElapsedTime(&ms, e[0], e[1]) == cudaSuccess) { h->stage_ms[st] += ms; h->stage_n[st]++; }
       used = 0;
     }
@@ -735,25 +733,19 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     return (int)DFB_ERR_CUDA;
   };
   if ((e = cudaSetDevice(h->device)) != cudaSuccess) return cfail("cudaSetDevice");
-  if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
-  if ((e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
-  if ((e = cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
-  // Default priority.  On one GPU a high-priority localizer takes SM slots from the latency-bound lookup / gather
-  // kernels of the current step and costs ~4 %, measured.  Holding it back until the update stage starts (HBM-bound,
-  // short-lived CTAs) and then giving it the greatest priority put 91 % of its kernel time under the update, but the
-  // update grew from 3.05 to 3.75 ms: the two share HBM, and the step got 2.3 % slower (H100 SXM, 700 W).  The
-  // sharded store's worker stream does get priority.
-  if ((e = cudaStreamCreateWithFlags(&h->loc_stream, cudaStreamNonBlocking)) != cudaSuccess) return cfail("cudaStreamCreate");
-  for (auto& L : h->loc) {
-    if ((e = cudaEventCreateWithFlags(&L.done, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-    if ((e = cudaEventCreateWithFlags(&L.consumed, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-  }
-  if ((e = cudaEventCreateWithFlags(&h->ev_fm_done, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-  if ((e = cudaEventCreateWithFlags(&h->ev_auc_done, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-  for (auto& s : h->in) {
-    if ((e = cudaEventCreateWithFlags(&s.copied, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-    if ((e = cudaEventCreateWithFlags(&s.consumed, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-  }
+  // All four at the default priority, the localizer's loc_stream too.  On one GPU a high-priority localizer takes SM
+  // slots from the latency-bound lookup / gather kernels of the current step and costs ~4 %, measured.  Holding it
+  // back until the update stage starts (HBM-bound, short-lived CTAs) and then giving it the greatest priority put 91 %
+  // of its kernel time under the update, but the update grew from 3.05 to 3.75 ms: the two share HBM, and the step
+  // got 2.3 % slower (H100 SXM, 700 W).  The sharded store's worker stream does get priority.
+  for (Stream* s : {&h->stream, &h->copy_stream, &h->aux_stream, &h->loc_stream})
+    if ((e = s->create()) != cudaSuccess) return cfail("cudaStreamCreate");
+  for (Event* ev : {&h->loc[0].done, &h->loc[0].consumed, &h->loc[1].done, &h->loc[1].consumed, &h->ev_fm_done,
+                    &h->ev_auc_done, &h->in[0].copied, &h->in[0].consumed, &h->in[1].copied, &h->in[1].consumed,
+                    &h->ev_or[0], &h->ev_or[1]})
+    if ((e = ev->create()) != cudaSuccess) return cfail("cudaEventCreate");
+  for (auto& ev : h->ring_done)
+    if ((e = ev.create()) != cudaSuccess) return cfail("cudaEventCreate");
   Table& t = h->tab;
   t.max_keys = (uint64_t)table_capacity;
   t.cap = next_pow2(2 * t.max_keys);
@@ -771,21 +763,19 @@ int dfb_create(const char* const* keys, const char* const* vals, int n, dfb_hand
     dfb_destroy(h);
     return rc;
   }
-  if ((e = cudaMalloc(&t.state, sizeof(TableState))) != cudaSuccess) return cfail("cudaMalloc(state)");
-  if ((e = cudaMalloc(&t.prog, 2 * sizeof(DevProgress))) != cudaSuccess) return cfail("cudaMalloc(prog)");
+  if ((e = h->tab_state.alloc(sizeof(TableState))) != cudaSuccess) return cfail("cudaMalloc(state)");
+  if ((e = h->tab_prog.alloc(2 * sizeof(DevProgress))) != cudaSuccess) return cfail("cudaMalloc(prog)");
+  t.state = h->tab_state.as<TableState>();
+  t.prog = h->tab_prog.as<DevProgress>();
   if ((e = cudaMemset(t.prog, 0, 2 * sizeof(DevProgress))) != cudaSuccess) return cfail("cudaMemset(prog)");
-  if ((e = cudaHostAlloc(&h->h_prog, sizeof(DevProgress), cudaHostAllocDefault)) != cudaSuccess) return cfail("cudaHostAlloc");
-  if ((e = cudaHostAlloc(&h->h_nvals, sizeof(unsigned long long), cudaHostAllocDefault)) != cudaSuccess) return cfail("cudaHostAlloc");
+  if ((e = h->h_prog.alloc(1)) != cudaSuccess) return cfail("cudaHostAlloc");
+  if ((e = h->h_nvals.alloc(1)) != cudaSuccess) return cfail("cudaHostAlloc");
   memset(h->h_prog, 0, sizeof(DevProgress));
-  if ((e = cudaHostAlloc(&h->h_scal, 2 * sizeof(unsigned long long), cudaHostAllocDefault)) != cudaSuccess) return cfail("cudaHostAlloc");
-  if ((e = cudaHostAlloc(&h->h_or, 2 * sizeof(unsigned long long), cudaHostAllocDefault)) != cudaSuccess) return cfail("cudaHostAlloc");
-  for (auto& ev : h->ev_or)
-    if ((e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
-  if ((e = cudaHostAlloc(&h->h_ring, dfb_engine::kRing * sizeof(DevProgress), cudaHostAllocDefault)) != cudaSuccess) return cfail("cudaHostAlloc");
+  if ((e = h->h_scal.alloc(2)) != cudaSuccess) return cfail("cudaHostAlloc");
+  if ((e = h->h_or.alloc(2)) != cudaSuccess) return cfail("cudaHostAlloc");
+  if ((e = h->h_ring.alloc(dfb_engine::kRing)) != cudaSuccess) return cfail("cudaHostAlloc");
   memset(h->h_ring, 0, dfb_engine::kRing * sizeof(DevProgress));
   memset(&h->backlog, 0, sizeof(DevProgress));
-  for (auto& ev : h->ring_done)
-    if ((e = cudaEventCreateWithFlags(&ev, cudaEventDisableTiming)) != cudaSuccess) return cfail("cudaEventCreate");
   h->launches += launch_table_init(t, p.seed, h->stream);
   if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return cfail("table init");
   *out = h;
@@ -798,46 +788,8 @@ int dfb_destroy(dfb_handle h) {
   cudaDeviceSynchronize();
   if (h->frozen) dfbh::frozen_destroy(h->frozen);   // a frozen snapshot not released: its handle dangles from here
   h->frozen = nullptr;
-  if (h->shard) dfbh::shard_destroy(h);
-  for (auto& L : h->loc) {
-    DevBuf* lb[] = {&L.keys, &L.lidx, &L.cnt, &L.occ_sorted, &L.col_start, &L.col_end, &L.scal};
-    for (auto* b : lb) if (b->p) cudaFree(b->p);
-    if (L.done) cudaEventDestroy(L.done);
-    if (L.consumed) cudaEventDestroy(L.consumed);
-  }
-  if (h->loc_stream) cudaStreamDestroy(h->loc_stream);
-  DevBuf* bufs[] = {&h->u_wv, &h->l_rkeys, &h->l_skeys, &h->l_pay, &h->l_spay,
-                    &h->hot_map, &h->hot_info, &h->hot_part, &h->hot_ps, &h->hot_cnt, &h->l_tmp, &h->auc_tmp, &h->pxv, &h->p_row, &h->occ, &h->occ_sorted, &h->lidx_sorted, &h->col_start, &h->col_end,
-                    &h->keys, &h->cnt, &h->slot, &h->u_w, &h->u_vrow, &h->flags, &h->pos, &h->lens, &h->cub,
-                    &h->gw, &h->gxxp, &h->gV, &h->pred, &h->vals, &h->auc_k, &h->auc_v, &h->a_off, &h->a_idx,
-                    &h->a_val, &h->a_lab, &h->a_w, &h->a_wpos, &h->a_vpos, &h->a_pred, &h->a_grad, &h->scal,
-                    &h->hasv, &h->rV, &h->rcg, &h->nvals, &h->id_ok};
-  for (auto* b : bufs) if (b->p) cudaFree(b->p);
-  for (auto& s : h->in) {
-    DevBuf* ib[] = {&s.off, &s.idx, &s.val, &s.lab, &s.keys, &s.cnt, &s.ids};
-    for (auto* b : ib) if (b->p) cudaFree(b->p);
-    if (s.copied) cudaEventDestroy(s.copied);
-    if (s.consumed) cudaEventDestroy(s.consumed);
-  }
+  h->shard.reset();
   dfbh::capacity_destroy(h);
-  if (h->tab.state) cudaFree(h->tab.state);
-  if (h->tab.prog) cudaFree(h->tab.prog);
-  if (h->h_prog) cudaFreeHost(h->h_prog);
-  if (h->h_nvals) cudaFreeHost(h->h_nvals);
-  if (h->h_ring) cudaFreeHost(h->h_ring);
-  if (h->h_scal) cudaFreeHost(h->h_scal);
-  if (h->h_or) cudaFreeHost(h->h_or);
-  for (auto& ev : h->ev_or) if (ev) cudaEventDestroy(ev);
-  for (auto& ev : h->ring_done) if (ev) cudaEventDestroy(ev);
-  for (auto& ev : h->pev) if (ev) cudaEventDestroy(ev);
-  if (h->stream) cudaStreamDestroy(h->stream);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
-  if (h->aux_stream) cudaStreamDestroy(h->aux_stream);
-  if (h->ev_t0) cudaEventDestroy(h->ev_t0);
-  if (h->ev_t1) cudaEventDestroy(h->ev_t1);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->ev_fm_done) cudaEventDestroy(h->ev_fm_done);
-  if (h->ev_auc_done) cudaEventDestroy(h->ev_auc_done);
   delete h;
   return DFB_OK;
 }
@@ -1246,7 +1198,7 @@ int dfb_wait_step(dfb_handle h, dfb_progress* out) {
 
 }  // extern "C"
 int dfbh::join_streams(dfb_engine* h) {
-  if (!h->ev_join) DFB_CUDA(h, cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming));
+  if (!h->ev_join) DFB_CUDA(h, h->ev_join.create());
   cudaStream_t others[] = {h->copy_stream, h->aux_stream, h->loc_stream};
   for (cudaStream_t o : others) {
     DFB_CUDA(h, cudaEventRecord(h->ev_join, o));
@@ -1259,7 +1211,7 @@ extern "C" {
 int dfb_time_mark(dfb_handle h, int which) {
   if (!h) return DFB_ERR_INVALID;
   DFB_CUDA(h, cudaSetDevice(h->device));
-  if (!h->ev_t0) { DFB_CUDA(h, cudaEventCreate(&h->ev_t0)); DFB_CUDA(h, cudaEventCreate(&h->ev_t1)); }
+  if (!h->ev_t0) { DFB_CUDA(h, h->ev_t0.create(cudaEventDefault)); DFB_CUDA(h, h->ev_t1.create(cudaEventDefault)); }
   if (which == 0) {
     DFB_CUDA(h, cudaEventRecord(h->ev_t0, h->stream));
   } else {
@@ -1282,9 +1234,9 @@ int dfb_profile(dfb_handle h, int enable) {
   if (!h) return DFB_ERR_INVALID;
   DFB_CUDA(h, cudaSetDevice(h->device));
   if (enable && h->pev.empty()) {
-    h->pev.assign((size_t)dfb_engine::kProfRing * dfb_engine::kStages * 2, nullptr);
+    h->pev.resize((size_t)dfb_engine::kProfRing * dfb_engine::kStages * 2);
     h->pev_used.assign((size_t)dfb_engine::kProfRing * dfb_engine::kStages, 0);
-    for (auto& ev : h->pev) DFB_CUDA(h, cudaEventCreate(&ev));
+    for (auto& ev : h->pev) DFB_CUDA(h, ev.create(cudaEventDefault));
   }
   if (!enable && h->profile) DFB_TRY(prof_drain(h));
   h->profile = enable ? 1 : 0;
@@ -1364,6 +1316,20 @@ int dfbh::stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t n
   DFB_CUDA(h, cudaEventRecord(in.copied, cs));
   return 0;
 }
+int dfbh::stage_host_batch(dfb_engine* h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
+                           const float* label, bool need_label, dfb_engine::InSet** in_out, size_t* nnz_out) {
+  DFB_TRY(check_csr(h, nrows, offset));
+  if (need_label && nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
+  DFB_CUDA(h, cudaSetDevice(h->device));
+  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
+  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
+  auto& in = h->in[h->seq & 1];
+  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
+  in.pre_ids = nullptr;
+  *in_out = &in;
+  *nnz_out = nnz;
+  return 0;
+}
 using dfbh::stage_raw;
 extern "C" {
 
@@ -1384,14 +1350,10 @@ static int raw_async_impl(dfb_handle h, size_t nrows, const uint64_t* offset, co
                           const float* value, const float* label, int push_cnt, int is_train, bool exact_range) {
   if (!h) return DFB_ERR_INVALID;
   DFB_NOT_SCORE_ONLY(h, "dfb_train_step_raw");
-  DFB_TRY(check_csr(h, nrows, offset));
-  if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
-  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
-  auto& in = h->in[h->seq & 1];
-  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  dfb_engine::InSet* inp;
+  size_t nnz;
+  DFB_TRY(dfbh::stage_host_batch(h, nrows, offset, ids, value, label, true, &inp, &nnz));
+  dfb_engine::InSet& in = *inp;
   DFB_CUDA(h, cudaStreamWaitEvent(h->stream, in.copied, 0));
   int rc = step_raw_dev(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(),
                         value ? in.val.as<float>() : nullptr, in.lab.as<float>(), push_cnt, is_train, in.copied,
@@ -1407,13 +1369,10 @@ int dfb_predict_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset, co
   if (!h) return DFB_ERR_INVALID;
   if (h->shard)
     return h->fail(DFB_ERR_INVALID, "this engine holds one shard of a sharded model: predict with dfb_shard_predict_async");
-  DFB_TRY(check_csr(h, nrows, offset));
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
-  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
-  auto& in = h->in[h->seq & 1];
-  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  dfb_engine::InSet* inp;
+  size_t nnz;
+  DFB_TRY(dfbh::stage_host_batch(h, nrows, offset, ids, value, label, false, &inp, &nnz));
+  dfb_engine::InSet& in = *inp;
   DFB_CUDA(h, cudaStreamWaitEvent(h->stream, in.copied, 0));
   int rc = predict_dev(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
                        label ? in.lab.as<float>() : nullptr, in.copied);

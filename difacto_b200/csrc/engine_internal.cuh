@@ -3,6 +3,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <memory>
 #include <string>
 #include <utility>
 #include <vector>
@@ -10,15 +11,75 @@
 #include "../../include/difacto_b200.h"
 #include "dfb_internal.cuh"
 
+// Owning handles of the engine's CUDA resources: each releases what it holds when it is destroyed or created anew, so
+// no member needs a line in a release list.  They move; they do not copy.
 struct DevBuf {
   void* p = nullptr;
   size_t bytes = 0;
+  DevBuf() = default;
+  DevBuf(DevBuf&& o) noexcept : p(std::exchange(o.p, nullptr)), bytes(std::exchange(o.bytes, 0)) {}
+  DevBuf& operator=(DevBuf&& o) noexcept { std::swap(p, o.p); std::swap(bytes, o.bytes); return *this; }
+  ~DevBuf() { reset(); }
+  void reset() { if (p) cudaFree(p); p = nullptr; bytes = 0; }
+  cudaError_t alloc(size_t n) {
+    reset();
+    const cudaError_t e = cudaMalloc(&p, n);
+    if (e == cudaSuccess) bytes = n;
+    return e;
+  }
   template <typename T> T* as() const { return static_cast<T*>(p); }
+};
+
+struct Event {
+  cudaEvent_t e = nullptr;
+  Event() = default;
+  Event(Event&& o) noexcept : e(std::exchange(o.e, nullptr)) {}
+  Event& operator=(Event&& o) noexcept { std::swap(e, o.e); return *this; }
+  ~Event() { reset(); }
+  void reset() { if (e) cudaEventDestroy(e); e = nullptr; }
+  cudaError_t create(unsigned flags = cudaEventDisableTiming) { reset(); return cudaEventCreateWithFlags(&e, flags); }
+  operator cudaEvent_t() const { return e; }
+};
+
+// non-blocking; priority 0 is the default priority, lower numbers are higher priorities
+struct Stream {
+  cudaStream_t s = nullptr;
+  Stream() = default;
+  Stream(Stream&& o) noexcept : s(std::exchange(o.s, nullptr)) {}
+  Stream& operator=(Stream&& o) noexcept { std::swap(s, o.s); return *this; }
+  ~Stream() { reset(); }
+  void reset() { if (s) cudaStreamDestroy(s); s = nullptr; }
+  cudaError_t create(int priority = 0) {
+    reset();
+    return cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, priority);
+  }
+  operator cudaStream_t() const { return s; }
+};
+
+// n elements of pinned host memory
+template <typename T> struct PinnedHost {
+  T* p = nullptr;
+  PinnedHost() = default;
+  PinnedHost(PinnedHost&& o) noexcept : p(std::exchange(o.p, nullptr)) {}
+  PinnedHost& operator=(PinnedHost&& o) noexcept { std::swap(p, o.p); return *this; }
+  ~PinnedHost() { reset(); }
+  void reset() { if (p) cudaFreeHost(p); p = nullptr; }
+  cudaError_t alloc(size_t n, unsigned flags = cudaHostAllocDefault) {
+    reset();
+    return cudaHostAlloc(reinterpret_cast<void**>(&p), n * sizeof(T), flags);
+  }
+  operator T*() const { return p; }
+  T* operator->() const { return p; }
 };
 
 struct ShardState;   // shard.cu
 struct dfb_frozen_s; // checkpoint.cu
+struct ShardDeleter { void operator()(ShardState* sh) const; };   // shard.cu
 
+// Members release themselves in reverse declaration order: the shard (declared last) goes before the engine's
+// buffers, and the streams (declared first) go last.  Before that, dfb_destroy waits for the device and releases, in
+// this order, the frozen snapshot (on its own stream, reading a copy of the table), the shard, then the table and the
+// V-row pool (capacity_destroy: the table is freed in stream order on `stream`, which is still alive).
 struct dfb_engine {
   dfb::Params prm;
   int device = 0;
@@ -35,9 +96,10 @@ struct dfb_engine {
   long long shard_timeout_ms = 20000;
   int long_row_nnz = 1024;  // rows with at least this many nonzeros are walked by a whole CTA (k_fm_long); 0: off
   int hot_split = 256;      // occurrence lists longer than this are pre-reduced in chunks by separate warps (0: off)
-  cudaStream_t stream = nullptr, copy_stream = nullptr, aux_stream = nullptr;
-  cudaEvent_t ev_fm_done = nullptr, ev_auc_done = nullptr;
+  Stream stream, copy_stream, aux_stream, loc_stream;
+  Event ev_fm_done, ev_auc_done;
   dfb::Table tab;
+  DevBuf tab_state, tab_prog;           // own tab.state and tab.prog
   std::string err;
   std::vector<std::pair<std::string, std::string>> unknown;
   uint64_t launches = 0;
@@ -54,15 +116,14 @@ struct dfb_engine {
   struct LocSet {
     DevBuf keys, lidx, cnt, occ_sorted, col_start, col_end;
     DevBuf scal;                          // {OR of all reversed keys, number of unique keys} (u64 x 2)
-    cudaEvent_t done = nullptr, consumed = nullptr;
+    Event done, consumed;
     bool used = false;
     const unsigned long long* dU() const { return scal.as<unsigned long long>() + 1; }
   } loc[2];
   uint64_t loc_seq = 0;
-  cudaStream_t loc_stream = nullptr;
-  unsigned long long* h_scal = nullptr;   // pinned: {or_all, n_unique} of a synchronous localize
-  unsigned long long* h_or = nullptr;     // pinned ring [2]: or_all of earlier asynchronous localizes
-  cudaEvent_t ev_or[2] = {nullptr, nullptr};
+  PinnedHost<unsigned long long> h_scal;   // {or_all, n_unique} of a synchronous localize
+  PinnedHost<unsigned long long> h_or;     // ring [2]: or_all of earlier asynchronous localizes
+  Event ev_or[2];
   bool or_pending[2] = {false, false};
   uint64_t or_seq = 0;
   DevBuf a_off, a_idx, a_val, a_lab, a_w, a_wpos, a_vpos, a_pred, a_grad;
@@ -71,7 +132,7 @@ struct dfb_engine {
   // double-buffered inputs of the pipelined step
   struct InSet {
     DevBuf off, idx, val, lab, keys, cnt, ids;
-    cudaEvent_t copied = nullptr, consumed = nullptr;
+    Event copied, consumed;
     const void* pre_ids = nullptr;     // host batch already staged by dfb_prefetch_raw (identity check)
     const void* pre_lab = nullptr;
     size_t pre_nrows = 0, pre_nnz = 0;
@@ -82,8 +143,8 @@ struct dfb_engine {
   uint64_t seq = 0;
   // per-step Progress snapshots of the pipelined path (pinned ring + completion events)
   static constexpr int kRing = 8;
-  dfb::DevProgress* h_ring = nullptr;
-  cudaEvent_t ring_done[kRing] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+  PinnedHost<dfb::DevProgress> h_ring;
+  Event ring_done[kRing];
   uint64_t submitted = 0, collected = 0;
   dfb::DevProgress backlog;             // snapshots folded in when the ring was full
   // optional per-stage CUDA-event timing (bench.py's roofline numbers)
@@ -92,15 +153,14 @@ struct dfb_engine {
   static constexpr int kStages = DFB_NUM_STAGES;
   static constexpr int kProfRing = 32;
   int profile = 0;
-  std::vector<cudaEvent_t> pev;          // [kProfRing][kStages][2]
+  std::vector<Event> pev;                // [kProfRing][kStages][2]
   std::vector<char> pev_used;            // [kProfRing][kStages]
   uint64_t prof_steps = 0;
   double stage_ms[kStages] = {};
   uint64_t stage_n[kStages] = {};
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr, ev_join = nullptr;   // dfb_time_mark
-  dfb::DevProgress* h_prog = nullptr;   // pinned
-  unsigned long long* h_nvals = nullptr;  // pinned
-  ShardState* shard = nullptr;          // the NVLink-sharded store this engine is a rank of (shard.cu)
+  Event ev_t0, ev_t1, ev_join;           // dfb_time_mark
+  PinnedHost<dfb::DevProgress> h_prog;
+  PinnedHost<unsigned long long> h_nvals;
   dfb_frozen_s* frozen = nullptr;       // the snapshot dfb_snapshot_begin froze, until dfb_frozen_release
 
   // capacity growth up to table_capacity_max / V_capacity_max (growth.cu)
@@ -115,8 +175,8 @@ struct dfb_engine {
     // the last table counts the host knows, and the insertion bounds enqueued since: each inserting call enqueues a
     // copy of {n_keys, n_vrows} as they are before it into a pinned ring, read once its event has completed
     static constexpr int kRing = 8;
-    unsigned long long* h_st = nullptr;             // pinned [kRing][2]
-    cudaEvent_t ev[kRing] = {};
+    PinnedHost<unsigned long long> h_st;            // [kRing][2]
+    Event ev[kRing];
     uint64_t at_k[kRing] = {}, at_v[kRing] = {};    // the bound totals when the copy was enqueued
     uint64_t head = 0, seq = 0;                     // ring entries [head, seq) are in flight
     uint64_t known_k = 0, known_v = 0, known_at_k = 0, known_at_v = 0, total_k = 0, total_v = 0;
@@ -124,9 +184,9 @@ struct dfb_engine {
     // has stored the keys its owner received.  calls numbers the bounds added, so that a correction reaches exactly
     // the copies whose totals include the corrected bound.
     uint64_t calls = 0, at_call[kRing] = {}, known_at_call = 0;
-    unsigned long long* h_rcv = nullptr;            // pinned, mapped [kRing]: the received keys of one sharded step
+    PinnedHost<unsigned long long> h_rcv;           // mapped [kRing]: the received keys of one sharded step
     unsigned long long* d_rcv = nullptr;            // its device address
-    cudaEvent_t rev[kRing] = {};
+    Event rev[kRing];
     uint64_t r_call[kRing] = {}, r_worst[kRing] = {};
     bool r_v[kRing] = {};                           // the step's bound was added to the V rows' total too
     uint64_t rhead = 0, rseq = 0;                   // entries [rhead, rseq) are not yet exact
@@ -134,6 +194,7 @@ struct dfb_engine {
     uint64_t n_growths = 0, n_waits = 0;
   } grow;
   int shard_growth = 0;     // kwarg shard_growth: a growing engine may be a rank of the fused sharded store
+  std::unique_ptr<ShardState, ShardDeleter> shard;   // the NVLink-sharded store this engine is a rank of (shard.cu)
 
   // true when a step runs the specialised sorted kernels: the 16-byte-lane forward (0 <= V_dim <= 128) and,
   // when it trains, the atomic-free sorted gradient reduction
@@ -173,7 +234,7 @@ struct dfb_engine {
 
 // CUDA-event pair around one stage of a step (only while dfb_profile is on), on the stream the stage runs on
 struct StageTimer {
-  dfb_engine* h; int st; cudaStream_t s; cudaEvent_t* e = nullptr;
+  dfb_engine* h; int st; cudaStream_t s; const Event* e = nullptr;
   StageTimer(dfb_engine* h_, int st_, cudaStream_t s_ = nullptr) : h(h_), st(st_), s(s_ ? s_ : h_->stream) {
     if (!h->profile) return;
     const int r = (int)(h->prof_steps % dfb_engine::kProfRing);
@@ -210,6 +271,11 @@ int check_csr(dfb_engine* h, size_t nrows, const uint64_t* offset);
 // (label may be NULL: a predict step without labels)
 int stage_raw(dfb_engine* h, dfb_engine::InSet& in, size_t nrows, size_t nnz, const uint64_t* offset,
               const uint64_t* ids, const float* value, const float* label);
+// the prologue of every step on a host batch of raw ids: checks the batch (a label is required when need_label),
+// and stages it into the input set of the next submission, unless dfb_prefetch_raw staged this very batch there
+// (InSet::prefetched).  *in_out: that set; *nnz_out: the batch's non-zeros.
+int stage_host_batch(dfb_engine* h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
+                     const float* label, bool need_label, dfb_engine::InSet** in_out, size_t* nnz_out);
 int collect_one(dfb_engine* h, dfb::DevProgress* acc);
 // growth.cu: the table (h->tab.cap slots) and the V-row pool (h->tab.vcap rows mapped, grow.v_max reserved) at create,
 // and their release
@@ -240,7 +306,6 @@ void table_copy_free(dfb::Table* t, cudaStream_t s);   // stream-ordered on s
 void counts_known(dfb_engine* h, uint64_t n_keys, uint64_t n_vrows);
 void frozen_destroy(dfb_frozen_s* f);   // checkpoint.cu: frees the copy after its stream's work
 int drain(dfb_engine* h);               // checkpoint.cu: wait for everything enqueued on any of the handle's streams
-void shard_destroy(dfb_engine* h);      // shard.cu
 int shard_sync(dfb_engine* h);          // shard.cu: drain the shard's streams
 bool shard_step_open(const dfb_engine* h);   // shard.cu: a sharded step is begun and its phase 4 not yet enqueued
 }  // namespace dfbh

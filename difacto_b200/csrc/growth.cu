@@ -160,13 +160,13 @@ int dfbh::capacity_create(dfb_engine* h) {
     t.Vcg = t.vonly ? nullptr : t.V + t.ks;
   }
   if (g.on) {
-    DFB_CUDA(h, cudaHostAlloc(&g.h_st, 2 * dfb_engine::Growth::kRing * sizeof(unsigned long long), cudaHostAllocDefault));
-    for (auto& ev : g.ev) DFB_CUDA(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    DFB_CUDA(h, g.h_st.alloc(2 * dfb_engine::Growth::kRing));
+    for (auto& ev : g.ev) DFB_CUDA(h, ev.create());
   }
   if (g.on && h->shard_growth) {
-    DFB_CUDA(h, cudaHostAlloc(&g.h_rcv, dfb_engine::Growth::kRing * sizeof(unsigned long long), cudaHostAllocMapped));
+    DFB_CUDA(h, g.h_rcv.alloc(dfb_engine::Growth::kRing, cudaHostAllocMapped));
     DFB_CUDA(h, cudaHostGetDevicePointer(reinterpret_cast<void**>(&g.d_rcv), g.h_rcv, 0));
-    for (auto& ev : g.rev) DFB_CUDA(h, cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    for (auto& ev : g.rev) DFB_CUDA(h, ev.create());
   }
   return 0;
 }
@@ -192,10 +192,6 @@ void dfbh::capacity_destroy(dfb_engine* h) {
   g.vchunks.clear();
   g.vbase = 0; g.vmapped = 0;
   h->tab.V = h->tab.Vcg = nullptr;
-  if (g.h_st) cudaFreeHost(g.h_st);
-  for (auto& ev : g.ev) if (ev) cudaEventDestroy(ev);
-  if (g.h_rcv) cudaFreeHost(g.h_rcv);
-  for (auto& ev : g.rev) if (ev) cudaEventDestroy(ev);
 }
 
 namespace {

@@ -34,19 +34,18 @@ struct ShardState {
   int rank = 0, S = 1;
   ShardLayout lay;
   size_t Bcap = 0, Ncap = 0;
-  void* mailbox = nullptr;
+  DevBuf mailbox;
   void* peer[8] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool connected = false;
-  cudaStream_t w_stream = nullptr, f_stream = nullptr, l_stream = nullptr;
-  cudaEvent_t ev_struct[2] = {}, ev_part[2] = {}, ev_reduce[2] = {}, ev_auc[2] = {}, ev_upd[2] = {}, ev_fin[2] = {},
-              ev_lookup[2] = {};
-  cudaEvent_t ev_grow = nullptr;     // a rehash on stream O, which the lookup of the same step waits for
+  Stream w_stream, f_stream, l_stream;
+  Event ev_struct[2], ev_part[2], ev_reduce[2], ev_auc[2], ev_upd[2], ev_fin[2], ev_lookup[2];
+  Event ev_grow;                     // a rehash on stream O, which the lookup of the same step waits for
   uint64_t step = 0;
   dfb_engine::LocSet L;
   DevBuf wb, rowcnt, pred[2];    // wb: ShardBounds [2] by step parity (the AUC of step t reads it beside step t+1)
   DevBuf slot[2], conf[2];        // by step parity: the lookup of step t+1 runs beside the update of step t
   DevBuf w, vrow, wv, vsave, flags, ws;
-  DevProgress* dprog = nullptr;   // device: [0,S) per-worker scratch, [S,S+2) worker Progress by parity, [S+2,S+4) staging
+  DevBuf dprog;                   // DevProgress: [0,S) per-worker scratch, [S,S+2) worker Progress by parity, [S+2,S+4) staging
   long long timeout_cycles = 0;
   // the step being enqueued (dfb_shard_begin_* .. dfb_shard_phase(4))
   struct Ctx {
@@ -64,9 +63,9 @@ struct ShardState {
     LookupArgs la;
     bool auc = false;
   } cx;
-  DevProgress* src_prog(int r) { return dprog + r; }
-  DevProgress* prog_w(int d) { return dprog + S + d; }
-  DevProgress* stage(int d) { return dprog + S + 2 + d; }
+  DevProgress* src_prog(int r) { return dprog.as<DevProgress>() + r; }
+  DevProgress* prog_w(int d) { return dprog.as<DevProgress>() + S + d; }
+  DevProgress* stage(int d) { return dprog.as<DevProgress>() + S + 2 + d; }
   ShardBounds* bounds(int d) { return wb.as<ShardBounds>() + d; }
 };
 
@@ -91,7 +90,7 @@ bool dbg_on() {
 int shard_begin(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, const uint64_t* d_ids,
                 const float* d_val, const float* d_lab, int push_cnt, int is_train, cudaEvent_t inputs_ready,
                 cudaEvent_t consumed, bool predict = false, float* pred_out = nullptr) {
-  ShardState* shp = h->shard;
+  ShardState* shp = h->shard.get();
   if (!shp) return h->fail(DFB_ERR_INVALID, "dfb_shard_init was not called");
   ShardState& sh = *shp;
   if (!sh.connected) return h->fail(DFB_ERR_INVALID, "dfb_shard_connect was not called");
@@ -112,7 +111,7 @@ int shard_begin(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, 
 // 3 = O part 2, 4 = F.  A host thread that drives several engines of ONE device must interleave the phases
 // (phase p of every engine before phase p+1 of any), so that every wait refers to work enqueued earlier.
 int shard_phase(dfb_engine* h, int phase) {
-  ShardState* shp = h->shard;
+  ShardState* shp = h->shard.get();
   if (!shp || !shp->cx.open) return h->fail(DFB_ERR_INVALID, "no sharded step in progress (dfb_shard_begin_*)");
   ShardState& sh = *shp;
   ShardState::Ctx& c = sh.cx;
@@ -134,7 +133,7 @@ int shard_phase(dfb_engine* h, int phase) {
   const bool valued = d_val != nullptr;      // of THIS rank's batch; on the wire every batch is valued (kernels_shard.cu)
   const unsigned remote = ((1u << S) - 1u) & ~(1u << me);
   cudaStream_t W = sh.w_stream, O = h->stream, A = h->aux_stream, F = sh.f_stream, L = sh.l_stream;
-  void* mine = sh.mailbox;
+  void* mine = sh.mailbox.p;
   const size_t Kseg = lay.Kseg;
 
   const ShardHdr* hdr[8];
@@ -413,28 +412,10 @@ int shard_step(dfb_engine* h, size_t nrows, size_t nnz, const uint64_t* d_off, c
 
 }  // namespace
 
-void dfbh::shard_destroy(dfb_engine* h) {
-  ShardState* sh = h->shard;
-  if (!sh) return;
-  if (sh->w_stream) cudaStreamDestroy(sh->w_stream);
-  if (sh->f_stream) cudaStreamDestroy(sh->f_stream);
-  if (sh->l_stream) cudaStreamDestroy(sh->l_stream);
-  if (sh->ev_grow) cudaEventDestroy(sh->ev_grow);
-  cudaEvent_t* evs[] = {sh->ev_struct, sh->ev_part, sh->ev_reduce, sh->ev_auc, sh->ev_upd, sh->ev_fin, sh->ev_lookup};
-  for (auto* e : evs) for (int i = 0; i < 2; ++i) if (e[i]) cudaEventDestroy(e[i]);
-  DevBuf* bufs[] = {&sh->L.keys, &sh->L.lidx, &sh->L.cnt, &sh->L.occ_sorted, &sh->L.col_start, &sh->L.col_end, &sh->L.scal,
-                    &sh->wb, &sh->rowcnt, &sh->pred[0], &sh->pred[1], &sh->slot[0], &sh->slot[1], &sh->w, &sh->vrow, &sh->wv, &sh->conf[0],
-                    &sh->conf[1],
-                    &sh->vsave, &sh->flags, &sh->ws};
-  for (auto* b : bufs) if (b->p) cudaFree(b->p);
-  if (sh->dprog) cudaFree(sh->dprog);
-  if (sh->mailbox) cudaFree(sh->mailbox);
-  delete sh;
-  h->shard = nullptr;
-}
+void ShardDeleter::operator()(ShardState* sh) const { delete sh; }
 
 int dfbh::shard_sync(dfb_engine* h) {
-  ShardState* sh = h->shard;
+  ShardState* sh = h->shard.get();
   if (!sh) return DFB_OK;
   DFB_CUDA(h, cudaStreamSynchronize(sh->w_stream));
   DFB_CUDA(h, cudaStreamSynchronize(sh->l_stream));
@@ -472,8 +453,8 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
                                     "table_capacity_max = table_capacity and V_capacity_max = V_capacity, or with "
                                     "shard_growth = 1");
   DFB_CUDA(h, cudaSetDevice(h->device));
-  ShardState* sh = new ShardState();
-  h->shard = sh;
+  h->shard.reset(new ShardState());
+  ShardState* sh = h->shard.get();
   sh->rank = rank; sh->S = nranks; sh->Bcap = max_rows; sh->Ncap = max_nnz;
   // capacity of one (worker, owner) segment: everything for one rank, else twice the even share (skew margin)
   auto seg_default = [&](size_t total) { return nranks == 1 ? total : std::min(total, 2 * total / (size_t)nranks + 4096); };
@@ -481,24 +462,25 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
   const size_t Nseg = seg_nnz ? std::min(seg_nnz, max_nnz) : seg_default(max_nnz);
   sh->lay.compute(nranks, ks, max_rows, Kseg, Nseg);
   sh->timeout_cycles = h->shard_timeout_ms * 2000000LL;
-  auto fail = [&](int rc) { dfbh::shard_destroy(h); return rc; };
+  // a refused init leaves no shard: what it created so far is released with it
+  auto fail = [&](int rc) { h->shard.reset(); return rc; };
   cudaError_t e;
-  if ((e = cudaMalloc(&sh->mailbox, sh->lay.total)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMalloc(shard mailbox)"));
-  if ((e = cudaMemset(sh->mailbox, 0, sh->lay.total)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMemset(shard mailbox)"));
-  sh->peer[rank] = sh->mailbox;
+  if ((e = sh->mailbox.alloc(sh->lay.total)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMalloc(shard mailbox)"));
+  if ((e = cudaMemset(sh->mailbox.p, 0, sh->lay.total)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMemset(shard mailbox)"));
+  sh->peer[rank] = sh->mailbox.p;
   // the worker stream (localize / scatter of the NEXT step) and the lookup stream run beside the owner's update of
   // the current step on the engine's main stream: give them the higher priority, or the update's CTAs (queued
   // first) would take every SM slot that frees up and the overlap would not happen
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);
-  if ((e = cudaStreamCreateWithPriority(&sh->w_stream, cudaStreamNonBlocking, prio_hi)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
-  if ((e = cudaStreamCreateWithFlags(&sh->f_stream, cudaStreamNonBlocking)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
-  if ((e = cudaStreamCreateWithPriority(&sh->l_stream, cudaStreamNonBlocking, prio_hi)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
-  cudaEvent_t* evs[] = {sh->ev_struct, sh->ev_part, sh->ev_reduce, sh->ev_auc, sh->ev_upd, sh->ev_fin, sh->ev_lookup};
+  if ((e = sh->w_stream.create(prio_hi)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
+  if ((e = sh->f_stream.create()) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
+  if ((e = sh->l_stream.create(prio_hi)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaStreamCreate"));
+  Event* evs[] = {sh->ev_struct, sh->ev_part, sh->ev_reduce, sh->ev_auc, sh->ev_upd, sh->ev_fin, sh->ev_lookup};
   for (auto* ev : evs)
     for (int i = 0; i < 2; ++i)
-      if ((e = cudaEventCreateWithFlags(&ev[i], cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
-  if ((e = cudaEventCreateWithFlags(&sh->ev_grow, cudaEventDisableTiming)) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
+      if ((e = ev[i].create()) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
+  if ((e = sh->ev_grow.create()) != cudaSuccess) return fail(h->cuda_fail(e, "cudaEventCreate"));
   const size_t tot = (size_t)nranks * Kseg;
   // a scoring rank (score_only = 1) runs predict steps only: it has no InitV requests (flags, ws), no pull-time V rows
   // to save for the updates (conf, vsave) and no hot keys to pre-reduce.  Its mailbox is a training rank's: the peers
@@ -535,8 +517,8 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
         return fail(rc);
   }
   const size_t np = (size_t)nranks + 4;
-  if ((e = cudaMalloc(&sh->dprog, np * sizeof(DevProgress))) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMalloc"));
-  if ((e = cudaMemset(sh->dprog, 0, np * sizeof(DevProgress))) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMemset"));
+  if ((e = sh->dprog.alloc(np * sizeof(DevProgress))) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMalloc"));
+  if ((e = cudaMemset(sh->dprog.p, 0, np * sizeof(DevProgress))) != cudaSuccess) return fail(h->cuda_fail(e, "cudaMemset"));
   sh->connected = nranks == 1;
   if (mailbox_bytes) *mailbox_bytes = sh->lay.total;
   // cudaMemset of device memory is asynchronous: the zeroed mailbox must be in place before any peer may store into it
@@ -547,10 +529,10 @@ int dfb_shard_init(dfb_handle h, int rank, int nranks, size_t max_rows, size_t m
 int dfb_shard_export(dfb_handle h, void** mailbox_ptr, unsigned char* handle64) {
   if (!h || !h->shard) return DFB_ERR_INVALID;
   DFB_CUDA(h, cudaSetDevice(h->device));
-  if (mailbox_ptr) *mailbox_ptr = h->shard->mailbox;
+  if (mailbox_ptr) *mailbox_ptr = h->shard->mailbox.p;
   if (handle64) {
     cudaIpcMemHandle_t mh;
-    DFB_CUDA(h, cudaIpcGetMemHandle(&mh, h->shard->mailbox));
+    DFB_CUDA(h, cudaIpcGetMemHandle(&mh, h->shard->mailbox.p));
     memcpy(handle64, &mh, 64);
   }
   return DFB_OK;
@@ -594,14 +576,10 @@ int dfb_shard_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, con
                          const float* label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
   DFB_NOT_SCORE_ONLY(h, "dfb_shard_step_async");
-  DFB_TRY(dfbh::check_csr(h, nrows, offset));
-  if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
-  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
-  auto& in = h->in[h->seq & 1];
-  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  dfb_engine::InSet* inp;
+  size_t nnz;
+  DFB_TRY(dfbh::stage_host_batch(h, nrows, offset, ids, value, label, true, &inp, &nnz));
+  dfb_engine::InSet& in = *inp;
   int rc = shard_step(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
                       in.lab.as<float>(), push_cnt, is_train, in.copied, in.consumed);
   h->seq++;
@@ -620,15 +598,10 @@ int dfb_shard_begin_async(dfb_handle h, size_t nrows, const uint64_t* offset, co
                           const float* label, int push_cnt, int is_train) {
   if (!h) return DFB_ERR_INVALID;
   DFB_NOT_SCORE_ONLY(h, "dfb_shard_begin_async");
-  DFB_TRY(dfbh::check_csr(h, nrows, offset));
-  if (nrows && !label) return h->fail(DFB_ERR_INVALID, "label is NULL");
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
-  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
-  auto& in = h->in[h->seq & 1];
-  if (!(in.pre_ids == ids && ids && in.pre_nrows == nrows && in.pre_nnz == nnz))
-    DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  dfb_engine::InSet* inp;
+  size_t nnz;
+  DFB_TRY(dfbh::stage_host_batch(h, nrows, offset, ids, value, label, true, &inp, &nnz));
+  dfb_engine::InSet& in = *inp;
   int rc = shard_begin(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
                        in.lab.as<float>(), push_cnt, is_train, in.copied, in.consumed);
   h->seq++;
@@ -642,13 +615,10 @@ namespace {
 int shard_begin_predict(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids, const float* value,
                         const float* label, float* pred_out) {
   if (!h) return DFB_ERR_INVALID;
-  DFB_TRY(dfbh::check_csr(h, nrows, offset));
-  DFB_CUDA(h, cudaSetDevice(h->device));
-  const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
-  if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
-  auto& in = h->in[h->seq & 1];
-  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(dfbh::stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  dfb_engine::InSet* inp;
+  size_t nnz;
+  DFB_TRY(dfbh::stage_host_batch(h, nrows, offset, ids, value, label, false, &inp, &nnz));
+  dfb_engine::InSet& in = *inp;
   int rc = shard_begin(h, nrows, nnz, in.off.as<uint64_t>(), in.ids.as<uint64_t>(), value ? in.val.as<float>() : nullptr,
                        label ? in.lab.as<float>() : nullptr, 0, 0, in.copied, in.consumed, true, pred_out);
   h->seq++;

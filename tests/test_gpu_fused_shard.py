@@ -261,6 +261,29 @@ def test_fused_shard_rows_without_nonzeros_count():
     assert prog[1][1].nrows == 40 and prog[1][2].nrows == 40
 
 
+def test_fused_shard_begin_restages_a_prefetch_with_another_label():
+    """a batch prefetched with label array A and begun with the same ids but label array B trains on B: a prefetch is
+    reused only for the same pointers, label included.  Compared with a twin store stepped on B without a prefetch"""
+    (E,), (T,) = make_local(1, KW), make_local(1, KW)
+    off, ids, val, lab = batch_fn(0, 0)
+    flipped = -lab
+    for X in (E, T):          # a trained model, so that the two labelings give different losses and updates
+        enqueue_local([X], [(off, ids, val, lab)], True, True)
+        X.wait_step()
+    E.prefetch_raw(len(lab), off, ids, val, lab)
+    E.shard_begin_async(len(lab), off, ids, val, flipped)
+    for phase in range(5):
+        E.shard_phase(phase)
+    enqueue_local([T], [(off, ids, val, flipped)], False, True)
+    pe, pt = E.wait_step(), T.wait_step()
+    assert abs(pe.loss - pt.loss) <= 1e-5 * abs(pt.loss) + 1e-5, (pe.loss, pt.loss)
+    keys = np.unique(ids)
+    for a, b in zip(E.read_entries(keys), T.read_entries(keys)):
+        assert_close(a, b, what="prefetch with label A, step on label B", rtol=1e-5, atol=1e-6)
+    E.close()
+    T.close()
+
+
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs 2 GPUs (gpurun --gpus 2)")
 @pytest.mark.parametrize("big", [False, True])
 def test_fused_shard_two_gpus_one_process_vs_oracle_simulation(big):
