@@ -1163,7 +1163,7 @@ int dfb_train_step_async(dfb_handle h, size_t nrows, const uint64_t* offset, con
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !index) return h->fail(DFB_ERR_INVALID, "index is NULL");
   auto& in = h->in[h->seq & 1];
-  in.pre_ids = nullptr;
+  in.pre = {};
   cudaStream_t cs = h->copy_stream;
   // the copy of batch t+1 may overwrite set b only after batch t-1 (same set) was consumed
   if (h->seq >= 2) DFB_CUDA(h, cudaStreamWaitEvent(cs, in.consumed, 0));
@@ -1324,8 +1324,9 @@ int dfbh::stage_host_batch(dfb_engine* h, size_t nrows, const uint64_t* offset, 
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
   auto& in = h->in[h->seq & 1];
-  if (!in.prefetched(ids, label, nrows, nnz)) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = nullptr;
+  const bool reuse = in.prefetched(offset, ids, value, label, nrows, nnz);
+  in.pre = {};                                // (also when the staging below fails part way)
+  if (!reuse) DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
   *in_out = &in;
   *nnz_out = nnz;
   return 0;
@@ -1341,8 +1342,9 @@ int dfb_prefetch_raw(dfb_handle h, size_t nrows, const uint64_t* offset, const u
   const size_t nnz = nrows ? (size_t)offset[nrows] : 0;
   if (nnz && !ids) return h->fail(DFB_ERR_INVALID, "ids is NULL");
   auto& in = h->in[h->seq & 1];
+  in.pre = {};
   DFB_TRY(stage_raw(h, in, nrows, nnz, offset, ids, value, label));
-  in.pre_ids = ids; in.pre_lab = label; in.pre_nrows = nrows; in.pre_nnz = nnz;
+  in.pre = {offset, ids, value, label, nrows, nnz};
   return DFB_OK;
 }
 

@@ -133,11 +133,15 @@ struct dfb_engine {
   struct InSet {
     DevBuf off, idx, val, lab, keys, cnt, ids;
     Event copied, consumed;
-    const void* pre_ids = nullptr;     // host batch already staged by dfb_prefetch_raw (identity check)
-    const void* pre_lab = nullptr;
-    size_t pre_nrows = 0, pre_nnz = 0;
-    bool prefetched(const void* ids, const void* lab, size_t nrows, size_t nnz) const {
-      return pre_ids == ids && ids && pre_lab == lab && pre_nrows == nrows && pre_nnz == nnz;
+    // the host batch dfb_prefetch_raw staged into this set: every argument, so that a step reuses the copy only when
+    // it is given the very same arrays (a NULL value or label matches NULL alone).  ids == nullptr: none staged
+    struct Batch {
+      const void *off = nullptr, *ids = nullptr, *val = nullptr, *lab = nullptr;
+      size_t nrows = 0, nnz = 0;
+    } pre;
+    bool prefetched(const void* off, const void* ids, const void* val, const void* lab, size_t nrows, size_t nnz) const {
+      return ids && pre.ids == ids && pre.off == off && pre.val == val && pre.lab == lab && pre.nrows == nrows &&
+             pre.nnz == nnz;
     }
   } in[2];
   uint64_t seq = 0;

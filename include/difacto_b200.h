@@ -266,8 +266,11 @@ int dfb_train_step_raw_async(dfb_handle h, size_t nrows, const uint64_t* offset,
                              const float* value_or_null, const float* label, int push_cnt,
                              int is_train);
 /* optional double-buffering hint: start the H2D copy of the batch the NEXT dfb_train_step_raw_async call
- * (or dfb_predict_raw_async / sharded step) will be given (same pointers, label included; it may be NULL for a
- * predict step), so that the copy overlaps the step submitted before it */
+ * (or dfb_predict_raw_async / sharded step) will be given, so that the copy overlaps the step submitted before it.
+ * That step reuses the copy only when it is given the same nrows and the identical offset, ids, value and label
+ * arrays (the same pointers; a NULL value or label matches NULL only, and a label may be NULL for a predict step);
+ * otherwise it stages its own arguments as usual.  The contents of those arrays must not change between the
+ * prefetch and the step: the engine compares pointers, not contents. */
 int dfb_prefetch_raw(dfb_handle h, size_t nrows, const uint64_t* offset, const uint64_t* ids,
                      const float* value_or_null, const float* label);
 int dfb_train_step_raw_dev(dfb_handle h, size_t nrows, size_t nnz, const uint64_t* d_offset,
