@@ -235,10 +235,15 @@ class Reference:
     mode: "train", "val" (forward, loss, penalty; the batch's absent keys inserted when val_inserts) or "predict"
     (forward only).  mutant: one of MUTANTS, a deliberately wrong variant used to show the comparison's sharpness.
     hot_chunk: the chunk length of the hot-key mutants.  order: "sorted" or "generic", the forward kernel's summation
-    order (module docstring).  val_inserts: True for the reference and the plugin calls, False for the fused steps."""
+    order (module docstring).  val_inserts: True for the reference and the plugin calls, False for the fused steps.
+
+    streams: the InitV streams of a step whose keys are owned by S stores by key range (the sharded store): (bounds,
+    seeds), bounds[S + 1] cutting the batch's sorted keys into the owners' segments and seeds[S] each owner's rng state
+    before the step.  Each owner draws its own stream -- its count-push rows first, then its update's, each in
+    ascending key order over its own keys.  `seed` is then unused; None is one stream from `seed` over every key."""
 
     def __init__(self, batch, hp, pre, seed, push_cnt=False, mode="train", device="cpu", mutant=None, hot_chunk=256,
-                 budget=1 << 23, order="sorted", val_inserts=True):
+                 budget=1 << 23, order="sorted", val_inserts=True, streams=None):
         assert mutant is None or mutant in MUTANTS, mutant
         assert order in ("sorted", "generic"), order
         self.order, self.val_inserts = order, bool(val_inserts)
@@ -254,7 +259,13 @@ class Reference:
         self.keys, lidx, cnt = batch_keys(ids)
         self.U = Uk = len(self.keys)
         self.cnt = cnt
-        self.seed0 = int(seed)
+        if streams is None:
+            self.streams = [(0, Uk, int(seed))]
+        else:
+            bounds, seeds = streams
+            assert len(bounds) == len(seeds) + 1 and bounds[0] == 0 and bounds[-1] == Uk, (bounds, Uk)
+            self.streams = [(int(a), int(b), int(s)) for a, b, s in zip(bounds[:-1], bounds[1:], seeds)]
+        self.seed0 = self.streams[0][2]
         scal, hasv, V, cg = pre
         assert len(hasv) == Uk
         self.absent = hasv < 0
@@ -268,12 +279,13 @@ class Reference:
         if self.push and k > 0:
             self.push_initv = ~hv & (scal[:, 1] != 0) & (fea > np.float32(hp["V_threshold"]))
         self.n_push = int(self.push_initv.sum())
+        self.n_push_seg = [int(self.push_initv[a:b].sum()) for a, b, _ in self.streams]
         self.hv_pull = hv | self.push_initv
         Vp = np.where(hv[:, None], V, np.float32(0)).astype(np.float32) if k else np.zeros((Uk, 0), np.float32)
-        if self.n_push:
-            at, step = np.nonzero(self.push_initv)[0], max(1, budget // k)
-            for r0 in range(0, self.n_push, step):
-                Vp[at[r0:r0 + step]] = initv_rows(self.seed0, r0, len(at[r0:r0 + step]), k, hp["V_init_scale"],
+        for a, b, sd in self.streams:
+            at, step = a + np.nonzero(self.push_initv[a:b])[0], max(1, budget // max(k, 1))
+            for r0 in range(0, len(at), step):
+                Vp[at[r0:r0 + step]] = initv_rows(sd, r0, len(at[r0:r0 + step]), k, hp["V_init_scale"],
                                                   device).cpu().numpy()
         cgp = np.where(hv[:, None], cg, np.float32(0)).astype(np.float32) if k else Vp
         if mutant == "swap_tile_neighbour":        # a key's V row swapped with its successor's, mid-tile
@@ -566,6 +578,20 @@ def pen_partial_update_fast(num_sms):
     return m
 
 
+def pen_partial_bwd_worker(num_sms):
+    """k_bwd_update<K, VAL, APPLY = false> (kernels_table.cu:714-1060, launched by launch_bwd_dense at :1469): the
+    sharded store's worker emitting gradient rows at the exact widths, grid_warps(ceil(n / 32), 8, num_sms * 8), 32 keys
+    per warp iteration.  A lane adds pen_w of its own key (phase A), 0.5 V_l2 (v.x^2 + .. + v.w^2) of the key its group
+    holds in each of the K / 4 passes (phase B), and, on the first group, that term of every hot key (more than 64
+    occurrences; at most 32): 1 + K / 4 + 32 terms per iteration, four squares summed before they join, then the warp
+    sum (5 levels) and a double atomic"""
+    def m(n_keys, k):
+        tiles = -(-n_keys // 32)
+        it = -(-tiles // _grid_warps(tiles, num_sms))
+        return it * (1 + k // 4 + 32) + 4 + 5
+    return m
+
+
 def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC):
     """hold one step's result to the reference.  pre / post: the state of ref's keys before / after (read_entries
     layout); obs: dict with any of loss, penalty, auc, nrows, new_keys, new_vrows, n_keys_delta, n_vrows_delta,
@@ -623,7 +649,9 @@ def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC)
         if "new_vrows" in obs:
             R.exact("new_vrows", obs["new_vrows"] == 0, f"{obs['new_vrows']}")
         if "rng_after" in obs:
-            R.exact("rng", obs["rng_after"] == ref.seed0, f"{obs['rng_after']} vs {ref.seed0}")
+            got = _per_stream(R, ref, obs["rng_after"])
+            want = [sd for _, _, sd in ref.streams]
+            R.exact("rng", got == want, f"{got} vs {want}")
         return R
 
     # ---- training: every key against its bounds, in chunks ----
@@ -663,7 +691,7 @@ def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC)
     R.exact("ambiguous keys", R.n_amb <= R.amb_cap, f"{R.n_amb} > cap {R.amb_cap}")
     ref_k0 = 0
 
-    # ---- the InitV stream: count-push rows first, then the update's, each in ascending key order ----
+    # ---- the InitV streams (one per owner): count-push rows first, then the update's, each in ascending key order ----
     if k:
         upd = np.concatenate(new_rows) if new_rows else np.zeros(0, np.int64)
         n_new = ref.n_push + len(upd)
@@ -671,24 +699,36 @@ def check(ref, pre, post, obs, what="step", pen_partial=None, amb_frac=AMB_FRAC)
             R.exact("new_vrows", obs["new_vrows"] == n_new, f"{obs['new_vrows']} vs {n_new} new rows in the table")
         if "n_vrows_delta" in obs:
             R.exact("n_vrows", obs["n_vrows_delta"] == n_new, f"grew by {obs['n_vrows_delta']}, want {n_new}")
-        if "rng_after" in obs:
-            want = int(lcg_jump(ref.seed0, 3 * k * n_new)[0])
-            R.exact("rng", obs["rng_after"] == want, f"{obs['rng_after']} vs seed jumped by 3 V_dim {n_new} = {want}")
+        got_rng = _per_stream(R, ref, obs["rng_after"]) if "rng_after" in obs else None
         badv, first = 0, ""
         step = max(1, ref.budget // max(k, 1))          # the stream's rows in chunks of bounded size
-        for r0 in range(0, len(upd), step):
-            rows = upd[r0:r0 + step]
-            Vw = initv_rows(ref.seed0, ref.n_push + r0, len(rows), k, ref.hp["V_init_scale"], d).cpu().numpy()
-            if ref.mutant == "adagrad_on_new_initv":
-                Vw = _adagrad_fresh(ref.hp, Vw)
-            bad = np.nonzero(~((V1[rows] == Vw).all(1) & (cg1[rows] == 0).all(1)))[0]
-            if len(bad) and not badv:
-                first = f"key {int(keys[rows[bad[0]]]):#018x}: {V1[rows[bad[0]]][:4]} vs {Vw[bad[0]][:4]}"
-            badv += len(bad)
+        for j, ((a, b, sd), n_push) in enumerate(zip(ref.streams, ref.n_push_seg)):
+            mine = upd[(upd >= a) & (upd < b)]
+            if got_rng is not None:
+                n_s = n_push + len(mine)
+                want = int(lcg_jump(sd, 3 * k * n_s)[0])
+                R.exact("rng", got_rng[j] == want, f"stream {j}: {got_rng[j]} vs seed jumped by 3 V_dim {n_s} = {want}")
+            for r0 in range(0, len(mine), step):
+                rows = mine[r0:r0 + step]
+                Vw = initv_rows(sd, n_push + r0, len(rows), k, ref.hp["V_init_scale"], d).cpu().numpy()
+                if ref.mutant == "adagrad_on_new_initv":
+                    Vw = _adagrad_fresh(ref.hp, Vw)
+                bad = np.nonzero(~((V1[rows] == Vw).all(1) & (cg1[rows] == 0).all(1)))[0]
+                if len(bad) and not badv:
+                    first = f"key {int(keys[rows[bad[0]]]):#018x}: {V1[rows[bad[0]]][:4]} vs {Vw[bad[0]][:4]}"
+                badv += len(bad)
         R.exact("InitV values", badv == 0, f"{badv} of {len(upd)} new rows differ from the stream, first {first}")
     elif "rng_after" in obs:
-        R.exact("rng", obs["rng_after"] == ref.seed0, "")
+        got = _per_stream(R, ref, obs["rng_after"])
+        R.exact("rng", got == [sd for _, _, sd in ref.streams], "")
     return R
+
+
+def _per_stream(R, ref, rng_after):
+    """the observed rng state of every InitV stream: one value, or one per owner when the step has several streams"""
+    got = [int(x) for x in np.atleast_1d(np.asarray(rng_after, np.int64))]
+    R.exact("rng streams", len(got) == len(ref.streams), f"{len(got)} rng states for {len(ref.streams)} streams")
+    return (got + [None] * len(ref.streams))[:len(ref.streams)]
 
 
 def _adagrad_fresh(hp, V):

@@ -218,3 +218,59 @@ def test_validation_on_unseen_ids(val_inserts):
     F.check(F.Reference(b, hp, pre, M.seed(), False, "val", val_inserts=val_inserts), pre, post, obs).assert_ok()
     R = F.check(F.Reference(b, hp, pre, M.seed(), False, "val", val_inserts=not val_inserts), pre, post, obs)
     assert not R.ok(), R.summary()
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# one InitV stream per owner: one worker's step over S oracle owners (shard_sim)
+# ---------------------------------------------------------------------------------------------------------------------
+def owner_steps(S, steps, hp, batch_fn):
+    """every step of shard_sim.simulate with S owners: (batch, push, pre, post, streams, observed) for the batch of
+    worker 0, whose keys are all the owners receive (the other workers' batches are empty).  The state of the batch's
+    keys is the owners' merged in key order; each owner's rng state before the step seeds its own stream"""
+    import shard_sim
+    from difacto_b200.sharded import shard_bounds_np
+    out = []
+    for t in range(steps):
+        before = shard_sim.simulate(S, t, hp, batch_fn)
+        after = shard_sim.simulate(S, t + 1, hp, batch_fn)
+        off, idx, val, lab = batch_fn(0, t)
+        keys = F.batch_keys(idx)[0]
+        bounds = shard_bounds_np(keys, S)
+
+        def merged(shards):
+            parts = [oracle_state(shards[s].M, keys[bounds[s]:bounds[s + 1]]) for s in range(S)]
+            return tuple(np.concatenate([p[j] for p in parts]) for j in range(4))
+        seeds = [sh.M.seed() for sh in before[0]]
+        prog = after[2][t][0]
+        obs = dict(loss=float(prog[0]), penalty=float(prog[1]), rng_after=[sh.M.seed() for sh in after[0]],
+                   n_keys_delta=sum(a.M.size() - b.M.size() for a, b in zip(after[0], before[0])))
+        out.append(((off, lab, idx, val), t < 2, merged(before[0]), merged(after[0]), (bounds, seeds), obs))
+    return out
+
+
+@pytest.mark.parametrize("S", [2, 3, 8])
+def test_per_owner_initv_streams(S):
+    """the simulated sharded store with one worker: every step within the reference's bounds when each owner draws its
+    own stream, and rejected by the single-stream reference whenever two owners drew InitV rows"""
+    import shard_sim
+    hp = dict(hyper(8, S), V_threshold=1)
+    empty = (np.zeros(5, U64), np.zeros(0, U64), None, np.ones(4, np.float32))
+
+    def batch_fn(rank, step):
+        if rank:
+            return empty
+        return shard_sim.raw_batch(0, step, step % 2 == 1, B=80, ids=300, hot=True, seed=S)
+    rejected = 0
+    for t, (b, push, pre, post, streams, obs) in enumerate(owner_steps(S, 4, hp, batch_fn)):
+        ref = F.Reference(b, hp, pre, 0, push, "train", "cpu", streams=streams)
+        R = F.check(ref, pre, post, obs, what=f"S {S} step {t}")
+        R.assert_ok()
+        bounds = streams[0]
+        drew = [int(((post[1] == 1) & (pre[1] != 1))[bounds[s]:bounds[s + 1]].sum()) for s in range(S)]
+        print(f"{R.summary()}; new rows per owner {drew}")
+        if sum(d > 0 for d in drew) >= 2:
+            R1 = F.check(F.Reference(b, hp, pre, streams[1][0], push, "train", "cpu"), pre, post,
+                         dict(obs, rng_after=obs["rng_after"][0]), what="one stream")
+            assert not R1.ok() and any("InitV" in f for f in R1.fail), R1.summary()
+            rejected += 1
+    assert rejected >= 2

@@ -58,9 +58,10 @@ class PathRun(S.Run):
         self.pen = {"train": F.pen_partial_update_fast(sms) if k in EXACT else F.pen_partial_warp_per_key(sms),
                     "val": F.pen_partial_warp_per_key(sms)}      # k_penalty (engine.cu:385-386)
 
-    def hold(self, b, mode, push, pre, post, seed0, obs, order, pen, val_inserts, what, mutants=(), t_step=0.0):
+    def hold(self, b, mode, push, pre, post, seed0, obs, order, pen, val_inserts, what, mutants=(), t_step=0.0,
+             streams=None):
         ref = F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", hot_chunk=self.hot_chunk, order=order,
-                          val_inserts=val_inserts)
+                          val_inserts=val_inserts, streams=streams)
         t0 = time.perf_counter()
         R = F.check(ref, pre, post, obs, what=what, pen_partial=pen, amb_frac=self.amb_frac)
         print(f"{R.summary()}; engine {t_step:.2f} s, reference + comparison {time.perf_counter() - t0:.1f} s, "
@@ -70,7 +71,8 @@ class PathRun(S.Run):
         del ref
         for m in mutants:
             Rm = F.check(F.Reference(b, self.hp, pre, seed0, push, mode, "cuda", mutant=m, hot_chunk=self.hot_chunk,
-                                     order=order, val_inserts=val_inserts), pre, post, obs, what=m, pen_partial=pen)
+                                     order=order, val_inserts=val_inserts, streams=streams), pre, post, obs, what=m,
+                         pen_partial=pen)
             assert not Rm.ok(), f"the {m} variant of the reference accepts the engine's step ({what}): {Rm.summary()}"
             print(f"  {m} rejects it: {Rm.fail[0] if Rm.fail else Rm.summary()}")
         self.reports.append(R)
