@@ -36,7 +36,7 @@ EXPORTS = [
     "dfb_dev_fm_step_peer", "dfb_localize", "dfb_train_step_raw", "dfb_train_step_raw_async",
     "dfb_train_step_raw_dev", "dfb_prefetch_raw", "dfb_snapshot_size", "dfb_snapshot", "dfb_restore",
     "dfb_snapshot_write", "dfb_restore_read", "dfb_snapshot_begin", "dfb_frozen_write", "dfb_frozen_error",
-    "dfb_frozen_release", "dfb_id_range_get", "dfb_id_range_set", "dfb_prune",
+    "dfb_frozen_release", "dfb_id_range_get", "dfb_id_range_set", "dfb_prune", "dfb_prune_rare",
     "dfb_shard_init", "dfb_shard_export", "dfb_shard_connect", "dfb_shard_step_dev", "dfb_shard_step_async",
     "dfb_shard_info", "dfb_shard_begin_async", "dfb_shard_begin_dev", "dfb_shard_phase", "dfb_time_mark", "dfb_time_elapsed_ms",
     "dfb_predict_raw_async", "dfb_predict_raw_dev", "dfb_shard_predict_async", "dfb_shard_begin_predict_async",
@@ -122,6 +122,7 @@ def lib():
         L.dfb_id_range_get.argtypes = [vp, C.POINTER(C.c_int)]
         L.dfb_id_range_set.argtypes = [vp, C.c_int]
         L.dfb_prune.argtypes = [vp, C.c_float, C.POINTER(u64)]
+        L.dfb_prune_rare.argtypes = [vp, C.c_float, C.POINTER(u64), C.POINTER(u64)]
         L.dfb_shard_init.argtypes = [vp, C.c_int, C.c_int, sz, sz, sz, sz, C.POINTER(sz)]
         L.dfb_shard_export.argtypes = [vp, C.POINTER(vp), vp]
         L.dfb_shard_connect.argtypes = [vp, vp]
@@ -508,6 +509,13 @@ class Engine:
         n = C.c_uint64()
         self._ck(self.L.dfb_prune(self.h, float(max_count), C.byref(n)))
         return n.value
+
+    def prune_rare(self, max_count):
+        """drop every entry with fea_cnt <= max_count, V rows included, and compact the V-row pool (dfb_prune_rare),
+        between steps; returns (entries dropped, V rows freed)"""
+        n, v = C.c_uint64(), C.c_uint64()
+        self._ck(self.L.dfb_prune_rare(self.h, float(max_count), C.byref(n), C.byref(v)))
+        return n.value, v.value
 
     def restore_from(self, fileobj, part=0, nparts=1, shard=0, nshards=1, chunk_bytes=0):
         """restore (merge) one snapshot stream read from fileobj.read (dfb_restore_read); returns has_aux"""

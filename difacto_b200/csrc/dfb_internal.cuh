@@ -333,10 +333,31 @@ int launch_rst_seed(Table& t, unsigned seed, cudaStream_t s);
 // blocks.  count: tot[2] = {kept, dropped} and blk_kept[grid] (zeroed by the caller).  rebuild: the kept entries into
 // kept[n_kept] (n_kept = tot[0]), the slots emptied, the kept entries re-inserted, n_keys lowered by tot[1].
 int prune_grid(uint64_t cap);
+// rare (dfb_prune_rare): an entry is dropped when fea_cnt <= max_count alone, and tot[4] = {kept, dropped, kept V rows,
+// dropped V rows}
 int launch_prune_count(const Table& t, float max_count, int grid, unsigned long long* tot, unsigned* blk_kept,
-                       cudaStream_t s);
+                       cudaStream_t s, bool rare = false);
 int launch_prune_rebuild(Table& t, float max_count, int grid, const unsigned long long* tot, const unsigned* blk_kept,
                          Entry* kept, uint64_t n_kept, cudaStream_t s);
+// ---- dfb_prune_rare: the V-row pool's compaction over W = ceil(n_vrows / 32) bitmap words (DESIGN.md section 10.1)
+struct RareWs {
+  unsigned* bits;        // [W], zeroed by the caller
+  int* owner;            // [n_vrows - n_vkeep]: the workspace entry of each kept row at or above n_vkeep
+  unsigned *cnt, *at;    // [2W] each: holes and movers per word, and their exclusive scan
+  int* list;             // [n_list]: the holes' rows, then the movers' rows
+  size_t n_list;
+  void* tmp;             // rare_scan_tmp_bytes(W)
+  size_t tmp_bytes;
+  unsigned* bad;         // zeroed by the caller; set (and DFB_ERR_INVALID raised into t.prog) when a kept row is owned
+                         // twice or lies outside [0, n_vrows): then no row moves and n_vrows is not lowered
+};
+size_t rare_scan_tmp_bytes(size_t W);
+// the rare rebuild: the kept entries into kept[n_kept] and the slots emptied (as launch_prune_rebuild), then, when rows
+// were dropped (n_vkeep < n_vrows), every kept row at or above n_vkeep moved into a hole below it and its workspace
+// entry pointed there; the kept entries re-inserted; n_keys lowered by tot[1] and n_vrows by tot[3]
+int launch_prune_rare(Table& t, float max_count, int grid, const unsigned long long* tot, const unsigned* blk_kept,
+                      Entry* kept, uint64_t n_kept, uint64_t n_vrows, uint64_t n_vkeep, const RareWs& ws,
+                      cudaStream_t s);
 
 // ---- GPU localizer (kernels_localize.cu): Localizer::Compact + the CSC view from one radix sort ----
 size_t localize_sort_tmp_bytes(size_t nnz);

@@ -15,6 +15,7 @@ TARGETS = {
     "difacto_b200": ["src/main.cc", "src/sgd_learner.cc"],
     "host_tests": ["tests/host_tests.cc", "src/sgd_learner.cc"],
     "prune_settings_tests": ["tests/prune_settings_tests.cc", "src/sgd_learner.cc"],
+    "prune_rare_settings_tests": ["tests/prune_rare_settings_tests.cc", "src/sgd_learner.cc"],
     "batch_dump": ["tests/batch_dump.cc"],
 }
 

@@ -117,7 +117,9 @@ struct CheckpointState {
     return st;
   }
   /** throws naming the first setting that differs from `now`.  `later`: settings the record format gained after
-   * checkpoints were first written, with the value a record that lacks one stands for (the setting's default) */
+   * checkpoints were first written, with the value a record that lacks one stands for (the setting's default).  A
+   * setting of `later` may also be left out of `now` (it is recorded only away from its default): a checkpoint that
+   * records it at another value is refused by its name too */
   void CheckSettings(const std::vector<std::pair<std::string, std::string>>& now,
                      const std::vector<std::pair<std::string, std::string>>& later = {}) const {
     for (const auto& kv : now) {
@@ -128,6 +130,15 @@ struct CheckpointState {
       if (*saved != kv.second)
         throw Error("checkpoint_in: " + kv.first + " differs from the checkpoint's (" + kv.first + " = " + *saved +
                     " there, " + kv.second + " here)");
+    }
+    for (const auto& d : later) {
+      bool given = false;
+      for (const auto& kv : now) given = given || kv.first == d.first;
+      if (given) continue;
+      for (const auto& s : settings)
+        if (s.first == d.first && s.second != d.second)
+          throw Error("checkpoint_in: " + d.first + " differs from the checkpoint's (" + d.first + " = " + s.second +
+                      " there, " + d.second + " here)");
     }
   }
 

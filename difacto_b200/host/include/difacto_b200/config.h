@@ -102,6 +102,9 @@ struct SGDLearnerParam {
   // V row and fea_cnt <= prune_count (dfb_prune)
   long long prune_period = 0;
   float prune_count = 0;
+  // 1: the periodic prune drops every entry with fea_cnt <= prune_count, V rows included, and compacts the V-row pool
+  // (dfb_prune_rare); 0: only the entries that carry no weight (dfb_prune)
+  int prune_rare = 0;
 
   KWArgs InitAllowUnknown(const KWArgs& kwargs) {
     KWArgs remain;
@@ -131,6 +134,7 @@ struct SGDLearnerParam {
         else if (k == "checkpoint_period") checkpoint_period = std::stoll(v);
         else if (k == "prune_period") prune_period = std::stoll(v);
         else if (k == "prune_count") prune_count = std::stof(v);
+        else if (k == "prune_rare") prune_rare = std::stoi(v);
         else remain.push_back(kv);
       } catch (const std::logic_error&) {
         throw ParamError("Invalid Parameter format for " + k + " value='" + v + "'");
@@ -142,6 +146,7 @@ struct SGDLearnerParam {
     if (checkpoint_period > 0 && checkpoint_out.empty()) throw ParamError("checkpoint_period needs checkpoint_out");
     if (prune_period < 0) throw ParamError("prune_period must be >= 0");
     if (prune_count != prune_count) throw ParamError("prune_count must be a number");
+    if (prune_rare != 0 && prune_rare != 1) throw ParamError("prune_rare must be 0 or 1");
     return remain;
   }
 };

@@ -69,9 +69,10 @@ class SGDLearner : public Learner {
    * given): a checkpoint resumes only under the same settings */
   static std::vector<std::pair<std::string, std::string>> Settings(const SGDLearnerParam& p, const KWArgs& kwargs);
   /** the settings a checkpoint written before they existed does not record, with the value it ran under: the
-   * default, so such a checkpoint resumes under the defaults and is refused under anything else */
+   * default, so such a checkpoint resumes under the defaults and is refused under anything else.  prune_rare is
+   * recorded only when it is set, so a fingerprint at the defaults is the one older checkpoints hold */
   static std::vector<std::pair<std::string, std::string>> SettingsAddedLater() {
-    return {{"prune_period", "0"}, {"prune_count", "0"}};
+    return {{"prune_period", "0"}, {"prune_count", "0"}, {"prune_rare", "0"}};
   }
 
  protected:
@@ -93,7 +94,8 @@ class SGDLearner : public Learner {
   /** after a training minibatch per worker (every rank's step collected): counts it, then prunes and checkpoints
    * when their periods have come round, the prune first */
   void EndMinibatch();
-  /** prune_period: every rank drops its entries with w == 0, no V row and fea_cnt <= prune_count (dfb_prune) */
+  /** prune_period: every rank drops its entries with w == 0, no V row and fea_cnt <= prune_count (dfb_prune), or
+   * with prune_rare every entry with fea_cnt <= prune_count, V rows included (dfb_prune_rare) */
   void MaybePrune();
   /** a checkpoint when the period has come round.  The model is frozen on every GPU now; a helper thread writes it,
    * then the state record, then renames the pointer file */

@@ -78,6 +78,7 @@ std::vector<std::pair<std::string, std::string>> SGDLearner::Settings(const SGDL
     for (const auto& kv : kwargs) if (kv.first == k.name) v = kv.second;
     s.push_back(std::make_pair(std::string(k.name), k.is_float ? FloatSetting(v) : IntSetting(v)));
   }
+  if (p.prune_rare) s.push_back({"prune_rare", std::to_string(p.prune_rare)});   // (SettingsAddedLater)
   return s;
 }
 
@@ -707,23 +708,34 @@ void SGDLearner::EndMinibatch() {
 // every rank's table at the same boundary, after all ranks' steps: the prune waits for each engine's streams
 void SGDLearner::MaybePrune() {
   if (param_.prune_period <= 0 || pos_.minibatches % static_cast<uint64_t>(param_.prune_period) != 0) return;
-  uint64_t dropped = 0, n_keys = 0;
+  const bool rare = param_.prune_rare != 0;
+  const char* call = rare ? "dfb_prune_rare" : "dfb_prune";
+  uint64_t dropped = 0, freed = 0, n_keys = 0, n_vrows = 0;
   for (int r = 0; r < param_.num_gpus; ++r) {
     const auto& e = ShardEngine(r);
-    uint64_t d = 0, k = 0;
-    int rc = dfb_prune(e->handle(), param_.prune_count, &d);
+    uint64_t d = 0, f = 0, k = 0, v = 0;
+    auto prune = [&]() {
+      return rare ? dfb_prune_rare(e->handle(), param_.prune_count, &d, &f) : dfb_prune(e->handle(), param_.prune_count, &d);
+    };
+    int rc = prune();
     if (rc == DFB_ERR_CAPACITY && !frozen_.empty()) {    // no room for the workspace beside a checkpoint's device copy
       WaitCheckpoint();
-      rc = dfb_prune(e->handle(), param_.prune_count, &d);
+      rc = prune();
     }
-    e->Check(rc, "dfb_prune");
-    e->Check(dfb_table_stats(e->handle(), &k, nullptr, nullptr, nullptr), "dfb_table_stats");
+    e->Check(rc, call);
+    e->Check(dfb_table_stats(e->handle(), &k, &v, nullptr, nullptr), "dfb_table_stats");
     dropped += d;
+    freed += f;
     n_keys += k;
+    n_vrows += v;
   }
-  if (verbose)
-    printf("Prune: minibatch %llu, dropped %llu, n_keys %llu\n", static_cast<unsigned long long>(pos_.minibatches),
-           static_cast<unsigned long long>(dropped), static_cast<unsigned long long>(n_keys));
+  if (!verbose) return;
+  printf("Prune: minibatch %llu, dropped %llu, n_keys %llu", static_cast<unsigned long long>(pos_.minibatches),
+         static_cast<unsigned long long>(dropped), static_cast<unsigned long long>(n_keys));
+  if (rare)
+    printf(", V rows freed %llu, n_vrows %llu", static_cast<unsigned long long>(freed),
+           static_cast<unsigned long long>(n_vrows));
+  printf("\n");
 }
 
 void SGDLearner::MaybeCheckpoint() {

@@ -415,6 +415,21 @@ int dfb_id_range_set(dfb_handle h, int bits);
  * touched: DFB_ERR_CAPACITY when it cannot be had, and then nothing has changed.  Refused on a score_only = 1
  * engine (DFB_ERR_INVALID): prune the model where it is trained. */
 int dfb_prune(dfb_handle h, float max_count, uint64_t* n_dropped);
+/* The frequency filter of an embedding table: drops every entry with fea_cnt <= max_count, whatever w and V hold, and
+ * an entry that owns a V row gives that row back.  Unlike dfb_prune this changes predictions: a dropped key reads as
+ * absent (w = 0, no V row) from then on, and when it comes back it starts afresh (FTRL state zero, a new V row from
+ * InitV once it qualifies again).  Afterwards n_keys is lower by *n_dropped and n_vrows by *n_vrows_freed; every kept V
+ * row lies in [0, n_vrows), one per key, with its [V | cg] bytes (pad columns too) unchanged; every kept entry keeps
+ * its key, scalars and pad, and its vrow points at where its row now is.  The InitV random state and the capacities
+ * (table slots, V rows, the mapped pool) do not change: the freed slots and rows take new keys, InitV allocating at
+ * n_vrows as before.  A model pruned so trains exactly as one restored from its snapshot with the dropped records
+ * removed.  Between steps only, as dfb_prune: it waits for every stream of the handle, is DFB_ERR_INVALID during a
+ * sharded step, and is refused on a score_only engine; a frozen snapshot is a copy and keeps its bytes.  The table is
+ * rebuilt in place and the V-row pool compacted in place: the kept rows above the new n_vrows move into the freed rows
+ * below it.  Its workspaces -- 32 bytes per kept entry, and, when rows are dropped, about 1/4 byte per V row, 12 bytes
+ * per dropped row and a scan's scratch -- are taken before anything changes: DFB_ERR_CAPACITY when they cannot be
+ * had, and then nothing has changed. */
+int dfb_prune_rare(dfb_handle h, float max_count, uint64_t* n_dropped, uint64_t* n_vrows_freed);
 
 /* ---------------------------------------------------------------------------------
  * key-range sharding (multi-GPU).  ps-lite Postoffice::GetServerKeyRanges
